@@ -235,6 +235,10 @@ plp_status plp_stereo_compute_batch_dev(plp_ctx *ctx, const plp_orb *left, const
     int L = 0;
     while (L < kMaxLevels && plp_orb_get_pyramid(left, 0, L, &v0) == PLP_OK) ++L;
     PLP_REQUIRE(L >= 1, "no pyramid: run the extraction first");
+    // fill_levels derives the per-frame strides from frames 0 and 1 only: frames past either handle's last extraction
+    // would be read from stale pyramid memory
+    PLP_REQUIRE(plp_orb_get_pyramid(left, batch - 1, 0, &v0) == PLP_OK && plp_orb_get_pyramid(right, batch - 1, 0, &v0) == PLP_OK,
+                "batch exceeds the frames of the extractors' last extraction");
     D.num_levels = L;
     PLP_TRY(plp_orb_get_tables(left, D.scale_factors, D.inv_scale_factors, ls, ils, nk));
     PLP_TRY(fill_levels(left, right, batch, D));

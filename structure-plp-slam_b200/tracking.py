@@ -235,13 +235,20 @@ class FrontEnd:
         self.track(batch, margin)
 
     # -- results --------------------------------------------------------------------------------------
+    def _after_tracking(self):
+        """The downloads below run on the extraction stream; the tracking outputs are written on the tracking stream."""
+        if self.track_ctx is not self.ctx:
+            self.ctx.wait(self.track_ctx)
+
     def download_keypoints(self, batch: int):
+        self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
         kp = self.d_kp.download(KP_DTYPE, (self.max_batch, self.cap))[:batch]
         desc = self.d_desc.download(np.uint8, (self.max_batch, self.cap, 32))[:batch]
         return [(kp[b, :n[b]].copy(), desc[b, :n[b]].copy()) for b in range(batch)]
 
     def download_tracking(self, batch: int):
+        self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
         matched = self.d_matched.download(np.int32, (self.max_batch, self.cap))[:batch]
         return dict(matched=[matched[b, :n[b]].copy() for b in range(batch)],

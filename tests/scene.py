@@ -8,6 +8,21 @@ import numpy as np
 import synth
 
 Z0 = 4.0  # plane depth [m]
+# LM iteration counts are compared loosely.  An optimize() call ends when a step leaves the robust chi2 sum exactly
+# unchanged (rho == 0, g2o's "terminate").  After convergence that test compares sums whose last bits depend on the
+# summation order, which differs between the kernel's warp reductions and the oracle's sequential sums: one side stops,
+# the other keeps taking rejected or negligible steps until the trial's 10 iterations run out.  The pose agrees (1e-8
+# relative) but a frame's count can differ by up to 9 per trial, either way.  What is checked: a frame runs iterations
+# iff the oracle's does, and a batch's total is within LM_ITERS_TOTAL_TOL of the oracle's (plus LM_ITERS_SLACK, for
+# batches of a few frames).
+LM_ITERS_TOTAL_TOL, LM_ITERS_SLACK = 0.1, 20
+
+
+def check_lm_iters(got, want, what=""):
+    got, want = np.asarray(got, np.int64), np.asarray(want, np.int64)
+    assert np.array_equal(got == 0, want == 0), f"{what}: frames without LM iterations differ: {got} vs {want}"
+    assert abs(int(got.sum()) - int(want.sum())) <= LM_ITERS_TOTAL_TOL * want.sum() + LM_ITERS_SLACK, \
+        f"{what}: {got.sum()} LM iterations vs the oracle's {want.sum()}"
 
 
 class PlanarSequence:
@@ -70,3 +85,33 @@ class PlanarSequence:
         dT[:3, :3] = synth.so3_exp(xi[:3])
         dT[:3, 3] = xi[3:]
         return dT @ self.poses[t]
+
+
+def oracle_track(orc, plp, seq, res, t, T_pred, margin=20.0):
+    """The oracle chain of frame_tracker::motion_based_track for frame t of `seq`: match_current_and_last_frames
+    (retried with 2 x margin below 20 matches) -> pose_optimize -> discard_outliers.  res[t - 1] / res[t] are oracle
+    ORB extractions; plp is the package (only its ctypes structures are used).
+    Returns (matched, pose, num_valid, n_inliers, LM iterations)."""
+    import oracle_api
+    grid = plp.capi.make_grid(seq.cols, seq.rows)
+    cam = plp.capi.make_camera(synth.FX, synth.FY, synth.CX, synth.CY, seq.cols, seq.rows)
+    sf, isig = synth.scale_factors(), synth.inv_level_sigma_sq()
+    last = seq.last_frame_landmarks(t - 1, res[t - 1]["kps"], res[t - 1]["desc"])
+    k = res[t]["kps"]
+    curr = dict(x=k["x"], y=k["y"], octave=k["octave"], angle=k["angle"], desc=res[t]["desc"])
+    # module/frame_tracker.cc:63-77
+    m, nm = orc.match_current_and_last_frames(grid, sf, cam, curr, T_pred, seq.poses[t - 1], last, margin, True)
+    if nm < 20:
+        m, nm = orc.match_current_and_last_frames(grid, sf, cam, curr, T_pred, seq.poses[t - 1], last, 2 * margin, True)
+    if nm < 20:  # no pose optimisation: the tracker reports 0 LM iterations
+        return np.full(len(k), -1, np.int32), T_pred, 0, 0, 0
+    idx = np.nonzero(m >= 0)[0]
+    pts = np.zeros(len(idx), oracle_api.PT_OBS_DTYPE)
+    pts["pos_w"] = last["pos_w"][m[idx]]
+    pts["obs_x"], pts["obs_y"] = k["x"][idx], k["y"][idx]
+    pts["x_right"] = -1.0
+    pts["inv_sigma_sq"] = isig[k["octave"][idx]]
+    T, pout, _, n_inl, iters = orc.pose_optimize(cam, T_pred, pts)
+    m = m.copy()
+    m[idx[pout != 0]] = -1  # discard_outliers (frame_tracker.cc:253-283)
+    return m, T, int((m >= 0).sum()), n_inl, iters
