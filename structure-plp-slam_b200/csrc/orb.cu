@@ -95,6 +95,60 @@ __device__ __forceinline__ const uint8_t *level_ptr(const OrbDev &P, int b, int 
 }
 __device__ __forceinline__ int level_pitch(const OrbDev &P, int l) { return l == 0 ? (int)P.img0_step : P.lv[l].pitch; }
 
+// ---- TMA staging of pyramid tiles (Gaussian blur and FAST) -----------------------------------------------------------
+// Every level is described as an (x, y, frame) uint8 tensor (plp_orb::maps) with one box shape, kBoxW x kBoxH x 1: the
+// source box of a 64 x 32 blur tile.  The innermost coordinate of a tiled copy must be a multiple of 16 BYTES (an
+// unaligned x is an illegal instruction); any y -- negative included -- is accepted, and out-of-image elements arrive
+// as zeros.
+constexpr int kBtW = 64, kBtH = 32;  // blur output tile
+constexpr int kBoxW = 96, kBoxH = kBtH + 6, kBoxX = 16;  // the box starts kBoxX columns left of the blur tile
+static_assert(kBoxW >= kBoxX + kBtW + 3 && kBoxW % 16 == 0 && kBoxX % 16 == 0 && kBtW % 16 == 0,
+              "TMA box: 16-byte aligned start and extent covering the 3-pixel halo");
+static_assert(kBoxH % 2 == 0 && kBtH % 2 == 0, "the blur passes work on pairs of rows");
+constexpr int kBoxStage = (kBoxH * kBoxW + 127) & ~127;  // a box in a shared-memory ring (TMA destinations: 128-byte aligned)
+
+struct BlurMaps {
+    CUtensorMap m[kMaxLevels];
+};
+
+__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
+
+// the descriptor of level l: a kernel parameter (__grid_constant__) or, with PLP_TMA_MAPS=global, an array in device
+// memory (acquired through the tensormap proxy, since the level-0 entry is rewritten when the caller's buffer changes)
+template <bool kMapsInGlobal>
+__device__ __forceinline__ const CUtensorMap *level_map(const BlurMaps &M, const CUtensorMap *gmaps, int l) {
+    const CUtensorMap *tm = kMapsInGlobal ? gmaps + l : &M.m[l];
+    if (kMapsInGlobal) asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(tm) : "memory");
+    return tm;
+}
+
+__device__ __forceinline__ void mbar_init(uint32_t bar) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar)); }
+
+// bounded wait for phase `parity` of an mbarrier; false if it did not complete (the copy never arrived)
+__device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity) {
+    uint32_t done = 0;
+    for (int spin = 0; spin < (1 << 14) && !done; ++spin)
+        asm volatile(
+            "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+            : "=r"(done)
+            : "r"(bar), "r"(parity)
+            : "memory");
+    return done != 0;
+}
+
+// thread 0 arms `bar` for `bytes` of copies of the current phase (before issuing them)
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+
+// one box at (x, y, frame) of tensor `tm` into shared memory at `dst` (128-byte aligned), completing on `bar`
+__device__ __forceinline__ void tma_box_load(uint32_t dst, const CUtensorMap *tm, int x, int y, int f, uint32_t bar) {
+    asm volatile(
+        "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+        ::"r"(dst), "l"(tm), "r"(x), "r"(y), "r"(f), "r"(bar)
+        : "memory");
+}
+
 // =====================================================================================================
 // 1. pyramid: cv::resize(INTER_LINEAR) fixed-point model (SURVEY.md Appendix A.1)
 // =====================================================================================================
@@ -1057,157 +1111,165 @@ __device__ __forceinline__ float util_sin(float v) {
 
 // cv::GaussianBlur(level, 7x7, sigma 2, BORDER_REFLECT_101) of every pyramid level (orb_extractor.cc:148-149) in
 // OpenCV's fixed-point form: Q8 kernel [18 34 48 56 48 34 18], exact integer passes, (v + 32768) >> 16.
-// One CTA per 64 x 32 output tile: 70 x 38 source tile -> smem, horizontal pass (u16), vertical pass, 32-bit stores.
-constexpr int kBtW = 64, kBtH = 32;
-__global__ void __launch_bounds__(256) blur_tiles_kernel(OrbDev P) {
-    __shared__ __align__(16) uint8_t s_src[(kBtH + 6) * 72];
-    __shared__ __align__(16) unsigned short s_h[(kBtH + 6) * kBtW];
+// A 64 x 32 output tile is made from a kBoxW x kBoxH source box in shared memory (box column kBoxX = tile column 0, box
+// row 3 = tile row 0): horizontal pass into vertically paired u16 sums, vertical pass, 32-bit stores.  Two kernels fill
+// the box: blur_tiles_tma_kernel by TMA bulk tensor copies, blur_tiles_kernel (buffers TMA cannot describe) by plain loads.
+
+// horizontal pass: h2[rp * kBtW + x] = h(2 rp, x) | h(2 rp + 1, x) << 16, where h(py, x) is the 7-tap sum of box row py
+// around output column x (<= 255 * 256, a u16).  Output x uses box bytes x + 13 .. x + 19 (image columns x0 + x - 3 ..
+// x0 + x + 3); for the outputs 4j .. 4j + 3 that is byte 1 of word j + 3 up to byte 2 of word j + 5, weighted by DP4A with
+// (18, 34, 48, 56) and (48, 34, 18, 0) after funnel shifts.  A thread makes 2 rows x 4 columns.
+__device__ __forceinline__ void blur_row4(const uint32_t *w, uint32_t h[4]) {
+    const uint32_t A = w[0], B = w[1], C = w[2];
+    const uint32_t kW1 = 0x38302212u, kW2 = 0x00122230u;  // bytes (18, 34, 48, 56) and (48, 34, 18, 0)
+    h[0] = __dp4a(__funnelshift_r(A, B, 8), kW1, __dp4a(__funnelshift_r(B, C, 8), kW2, 0u));
+    h[1] = __dp4a(__funnelshift_r(A, B, 16), kW1, __dp4a(__funnelshift_r(B, C, 16), kW2, 0u));
+    h[2] = __dp4a(__funnelshift_r(A, B, 24), kW1, __dp4a(__funnelshift_r(B, C, 24), kW2, 0u));
+    h[3] = __dp4a(B, kW1, __dp4a(C, kW2, 0u));
+}
+__device__ __forceinline__ void blur_h_pass(const uint8_t *box, uint32_t *h2) {
+    const uint32_t *src32 = reinterpret_cast<const uint32_t *>(box);
+    for (int i = threadIdx.x; i < (kBoxH / 2) * (kBtW / 4); i += blockDim.x) {
+        const int rp = i / (kBtW / 4), j = i % (kBtW / 4);
+        const uint32_t *w = src32 + 2 * rp * (kBoxW / 4) + j + (kBoxX - 4) / 4;
+        uint32_t e[4], o[4];
+        blur_row4(w, e);
+        blur_row4(w + kBoxW / 4, o);
+        *reinterpret_cast<uint4 *>(h2 + rp * kBtW + 4 * j) =
+            make_uint4(__byte_perm(e[0], o[0], 0x5410), __byte_perm(e[1], o[1], 0x5410), __byte_perm(e[2], o[2], 0x5410),
+                       __byte_perm(e[3], o[3], 0x5410));
+    }
+}
+
+// vertical pass: output rows 2q and 2q + 1 read the pairs q .. q + 3.  With the weights of an output row taken as byte
+// pairs, a pixel is four DP2A (u16 pair x u8 pair) into one 32-bit sum started at OpenCV's rounding constant:
+//   even row  (18, 34) (48, 56) (48, 34) (18, 0)        odd row  (0, 18) (34, 48) (56, 48) (34, 18)
+// The sum is at most 65280 * 256 + 32768 < 2^24, so it is exact and its byte 2 is (acc + 32768) >> 16.  A thread makes
+// 2 rows x 4 columns: the 256 threads of the CTA cover the tile in one go.
+constexpr int kBlurThreads = 256;
+static_assert((kBtH / 2) * (kBtW / 4) == kBlurThreads, "one vertical-pass job per thread");
+__device__ __forceinline__ void blur_v_pass(const uint32_t *h2, uint8_t *dst, int dpitch, int x0, int y0, int W, int H) {
+    const int q = threadIdx.x / (kBtW / 4), px = (threadIdx.x % (kBtW / 4)) * 4;
+    const int y = y0 + 2 * q;
+    if (y >= H || x0 + px >= W) return;
+    uint32_t r[4][4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const uint4 v = *reinterpret_cast<const uint4 *>(h2 + (q + k) * kBtW + px);
+        r[k][0] = v.x;
+        r[k][1] = v.y;
+        r[k][2] = v.z;
+        r[k][3] = v.w;
+    }
+    auto row = [&](uint32_t k0, uint32_t k1, uint32_t k2, uint32_t k3) -> uint32_t {
+        uint32_t a[4];
+#pragma unroll
+        for (int c = 0; c < 4; ++c)
+            a[c] = __dp2a_lo(r[0][c], k0, __dp2a_lo(r[1][c], k1, __dp2a_lo(r[2][c], k2, __dp2a_lo(r[3][c], k3, 32768u))));
+        return __byte_perm(__byte_perm(a[0], a[1], 0x0062), __byte_perm(a[2], a[3], 0x0062), 0x5410);
+    };
+    // pitch is a multiple of 64: aligned 4-byte stores; bytes past the image width are padding
+    uint8_t *d = dst + (size_t)y * dpitch + x0 + px;
+    *reinterpret_cast<uint32_t *>(d) = row(0x2212u, 0x3830u, 0x2230u, 0x0012u);
+    if (y + 1 < H) *reinterpret_cast<uint32_t *>(d + dpitch) = row(0x1200u, 0x3022u, 0x3038u, 0x1222u);
+}
+
+// plain loads, one tile per CTA: the box columns the horizontal pass reads (kBoxX - 4 .. kBoxX + kBtW + 3) are gathered
+// with BORDER_REFLECT_101 applied to the coordinates
+__global__ void __launch_bounds__(kBlurThreads) blur_tiles_kernel(OrbDev P) {
+    __shared__ __align__(16) uint8_t s_src[kBoxH * kBoxW];
+    __shared__ __align__(16) uint32_t s_h2[(kBoxH / 2) * kBtW];
     const int b = blockIdx.y, tid = threadIdx.x;
     const BlurTile t = P.blur_tiles[blockIdx.x];
     const int l = t.level, W = P.lv[l].w, H = P.lv[l].h;
     const uint8_t *img = level_ptr(P, b, l);
     const int pitch = level_pitch(P, l);
-    for (int i = tid; i < (kBtH + 6) * 70; i += 256) {
-        const int py = i / 70, px = i - py * 70;
-        // rows / columns past the image edge + 3 only feed outputs that are never stored: clamp before reflecting
-        const int gy = reflect101(min(t.y0 - 3 + py, H + 2), H), gx = reflect101(min(t.x0 - 3 + px, W + 2), W);
-        s_src[py * 72 + px] = img[(size_t)gy * pitch + gx];
+    constexpr int kCols = kBtW + 8;
+    for (int i = tid; i < kBoxH * kCols; i += kBlurThreads) {
+        const int py = i / kCols, px = i - py * kCols;
+        // rows / columns past the image edge + 3 only feed outputs that are never stored, and box column kBoxX - 4 only
+        // meets DP4A weight 0: clamp before reflecting
+        const int gy = reflect101(min(t.y0 - 3 + py, H + 2), H);
+        const int gx = reflect101(min(max(t.x0 - 4 + px, -3), W + 2), W);
+        s_src[py * kBoxW + kBoxX - 4 + px] = img[(size_t)gy * pitch + gx];
     }
     __syncthreads();
-    for (int i = tid; i < (kBtH + 6) * kBtW; i += 256) {
-        const int py = i / kBtW, px = i - py * kBtW;
-        const uint8_t *s = s_src + py * 72 + px;
-        s_h[i] = (unsigned short)(18 * (s[0] + s[6]) + 34 * (s[1] + s[5]) + 48 * (s[2] + s[4]) + 56 * s[3]);
-    }
+    blur_h_pass(s_src, s_h2);
     __syncthreads();
-    uint8_t *dst = P.blur + (size_t)b * P.blur_frame_bytes + P.lv[l].blur_offset;
-    const int dpitch = P.lv[l].pitch;
-    for (int i = tid; i < kBtH * kBtW / 4; i += 256) {
-        const int py = i / (kBtW / 4), px = (i - py * (kBtW / 4)) * 4;
-        if (t.y0 + py >= H || t.x0 + px >= W) continue;
-        uint32_t packed = 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const unsigned short *h = s_h + py * kBtW + px + k;
-            const unsigned acc = 18u * (h[0] + h[6 * kBtW]) + 34u * (h[kBtW] + h[5 * kBtW]) + 48u * (h[2 * kBtW] + h[4 * kBtW]) +
-                                 56u * h[3 * kBtW];
-            packed |= ((acc + 32768u) >> 16) << (8 * k);
-        }
-        // pitch is a multiple of 64: aligned 4-byte store; bytes past the image width are padding
-        *reinterpret_cast<uint32_t *>(dst + (size_t)(t.y0 + py) * dpitch + t.x0 + px) = packed;
-    }
+    blur_v_pass(s_h2, P.blur + (size_t)b * P.blur_frame_bytes + P.lv[l].blur_offset, P.lv[l].pitch, t.x0, t.y0, W, H);
 }
 
-// ---- the same blur with the source tile staged by TMA and the passes on byte / half-word SIMD ---------------------
-// One CTA per 64 x 32 output tile.  (1) ONE bulk tensor copy (cp.async.bulk.tensor.3d, box 96 x 38 x 1 of the
-// (x, y, frame) tensor of the level) completes on an mbarrier -- no per-byte address arithmetic, no loads issued by the
-// SMs.  The innermost coordinate of a tiled copy must be a multiple of 16 BYTES (an
-// unaligned x is an illegal instruction, any y -- negative included -- is accepted, out-of-image elements arrive as
-// zeros), so the box is the 16-byte aligned superset [x0 - 16, x0 + 80) of the 70 columns the tile needs.
-// (2) tiles that touch the image border rebuild BORDER_REFLECT_101 inside shared memory (the mirrored pixels are part of
-// the same box).  (3) horizontal pass: a thread makes 4 outputs from 3 words with funnel shifts and DP4A
-// ([18 34 48 56] . bytes + [48 34 18 0] . bytes); (4) vertical pass on the u16 rows; OpenCV's rounding (v + 32768) >> 16.
-struct BlurMaps {
-    CUtensorMap m[kMaxLevels];
-};
-constexpr int kBoxW = 96, kBoxH = kBtH + 6, kBoxX = 16;  // the box starts kBoxX columns left of the tile
-static_assert(kBoxW >= kBoxX + kBtW + 3 && kBoxW % 16 == 0 && kBoxX % 16 == 0 && kBtW % 16 == 0,
-              "TMA box: 16-byte aligned start and extent covering the 3-pixel halo");
+// BORDER_REFLECT_101 inside a TMA box whose tile touches the image border (the mirrored pixels are part of the same box):
+// only the (at most) 3 + 3 halo columns and 3 + 3 halo rows the stored outputs read are rebuilt
+__device__ void blur_reflect_box(uint8_t *box, int bx0, int by0, int W, int H) {
+    for (int i = threadIdx.x; i < kBoxH * 6; i += blockDim.x) {
+        const int py = i / 6, k = i - py * 6;
+        const int gx = k < 3 ? k - 3 : W + (k - 3), gy = by0 + py;   // image columns -3 .. -1 and W .. W + 2
+        const int px = gx - bx0;
+        if (gy < 0 || gy >= H || px < 0 || px >= kBoxW) continue;
+        box[py * kBoxW + px] = box[py * kBoxW + (reflect101(gx, W) - bx0)];
+    }
+    __syncthreads();
+    for (int i = threadIdx.x; i < 6 * kBoxW; i += blockDim.x) {
+        const int k = i / kBoxW, px = i - k * kBoxW;
+        const int gy = k < 3 ? k - 3 : H + (k - 3);                  // image rows -3 .. -1 and H .. H + 2
+        const int py = gy - by0;
+        if (py < 0 || py >= kBoxH) continue;
+        box[py * kBoxW + px] = box[(reflect101(gy, H) - by0) * kBoxW + px];
+    }
+    __syncthreads();
+}
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
+// ---- the same blur with the source boxes staged by TMA, a run of tiles per CTA --------------------------------------
+// A CTA makes `run` consecutive tiles of one frame (the tile list is level-major, row-major inside a level).  Each box
+// arrives by ONE bulk tensor copy (box 96 x 38 x 1 of the (x, y, frame) tensor of the level, see tma_box_load) into a
+// two-stage shared-memory ring; every stage completes on its own mbarrier.  The copy of tile i + 1 is issued before tile
+// i is waited for, so it overlaps the passes of tile i.  The box is the 16-byte aligned superset [x0 - 16, x0 + 80) of
+// the 70 columns the tile needs; tiles that touch the image border rebuild BORDER_REFLECT_101 inside the box.
+// The grid is not persistent: short runs keep CTAs retiring, so that kernels of a concurrent higher-priority stream
+// (the tracking of the other sub-batch in the front end) still get SMs.
+// tiles per CTA: 4, 8 and 16 give the same blur time (0.34 ms per 256-frame sub-batch on one H100 80GB HBM3 at 400 W);
+// 4 gave the best step time of the front end, whose tracking stream needs SMs while the blur runs
+constexpr int kBlurRun = 4;
 template <bool kMapsInGlobal>
-__global__ void __launch_bounds__(256) blur_tiles_tma_kernel(const __grid_constant__ BlurMaps M, const CUtensorMap *gmaps, OrbDev P) {
-    __shared__ __align__(128) uint8_t s_src[kBoxH * kBoxW];
-    __shared__ __align__(16) unsigned short s_h[kBoxH * kBtW];
-    __shared__ __align__(8) unsigned long long s_bar;
+__global__ void __launch_bounds__(kBlurThreads) blur_tiles_tma_kernel(const __grid_constant__ BlurMaps M, const CUtensorMap *gmaps,
+                                                                      OrbDev P, int run) {
+    __shared__ __align__(128) uint8_t s_src[2][kBoxStage];
+    __shared__ __align__(16) uint32_t s_h2[(kBoxH / 2) * kBtW];
+    __shared__ __align__(8) unsigned long long s_bar[2];
     const int b = blockIdx.y, tid = threadIdx.x;
-    const BlurTile t = P.blur_tiles[blockIdx.x];
-    const int l = t.level, W = P.lv[l].w, H = P.lv[l].h;
-    const int bx0 = t.x0 - kBoxX, by0 = t.y0 - 3;  // image coordinates of box element (0, 0)
-    const uint32_t bar = smem_u32(&s_bar);
+    const int first = blockIdx.x * run, n = min(run, P.num_blur_tiles - first);
     if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar));
+        mbar_init(smem_u32(&s_bar[0]));
+        mbar_init(smem_u32(&s_bar[1]));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    if (tid == 0) {
-        // the descriptor: a kernel parameter (__grid_constant__) or, with PLP_TMA_MAPS=global, an array in device memory
-        // (acquired through the tensormap proxy, since the level-0 entry is rewritten when the caller's buffer changes)
-        const CUtensorMap *tm = kMapsInGlobal ? gmaps + l : &M.m[l];
-        if (kMapsInGlobal) asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(tm) : "memory");
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(kBoxH * kBoxW) : "memory");
-        asm volatile(
-            "cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
-            ::"r"(smem_u32(s_src)), "l"(tm), "r"(bx0), "r"(by0), "r"(b), "r"(bar)
-            : "memory");
-    }
-    {
-        uint32_t done = 0;
-        for (int spin = 0; spin < (1 << 14) && !done; ++spin)
-            asm volatile(
-                "{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                : "=r"(done)
-                : "r"(bar)
-                : "memory");
-        if (!done && tid == 0) P.status[b] = 3;  // the copy never completed: report it instead of hanging the device
-    }
-    if (t.x0 < 3 || by0 < 0 || t.x0 + kBtW + 3 > W || by0 + kBoxH > H) {  // BORDER_REFLECT_101 from inside the box
-        // only the (at most) 3 + 3 halo columns and 3 + 3 halo rows the stored outputs read are rebuilt
-        for (int i = tid; i < kBoxH * 6; i += 256) {
-            const int py = i / 6, k = i - py * 6;
-            const int gx = k < 3 ? k - 3 : W + (k - 3), gy = by0 + py;   // image columns -3 .. -1 and W .. W + 2
-            const int px = gx - bx0;
-            if (gy < 0 || gy >= H || px < 0 || px >= kBoxW) continue;
-            s_src[py * kBoxW + px] = s_src[py * kBoxW + (reflect101(gx, W) - bx0)];
-        }
+    auto issue = [&](int i) {  // thread 0: the box of tile first + i into stage i & 1
+        const BlurTile t = P.blur_tiles[first + i];
+        const uint32_t bar = smem_u32(&s_bar[i & 1]);
+        mbar_expect_tx(bar, kBoxH * kBoxW);
+        tma_box_load(smem_u32(s_src[i & 1]), level_map<kMapsInGlobal>(M, gmaps, t.level), t.x0 - kBoxX, t.y0 - 3, b, bar);
+    };
+    if (tid == 0) issue(0);
+    for (int i = 0; i < n; ++i) {
+        // every thread is past the passes of tile i - 1: its stage and s_h2 may be overwritten.  The stage was read and
+        // (border fix-up) written through the generic proxy, so the refill by the async proxy is ordered after a fence.
         __syncthreads();
-        for (int i = tid; i < 6 * kBoxW; i += 256) {
-            const int k = i / kBoxW, px = i - k * kBoxW;
-            const int gy = k < 3 ? k - 3 : H + (k - 3);                  // image rows -3 .. -1 and H .. H + 2
-            const int py = gy - by0;
-            if (py < 0 || py >= kBoxH) continue;
-            s_src[py * kBoxW + px] = s_src[(reflect101(gy, H) - by0) * kBoxW + px];
+        if (tid == 0 && i + 1 < n) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            issue(i + 1);
         }
+        const BlurTile t = P.blur_tiles[first + i];
+        const int l = t.level, W = P.lv[l].w, H = P.lv[l].h;
+        const int bx0 = t.x0 - kBoxX, by0 = t.y0 - 3;  // image coordinates of box element (0, 0)
+        uint8_t *box = s_src[i & 1];
+        // the copy never completed: report it instead of hanging the device
+        if (!mbar_wait(smem_u32(&s_bar[i & 1]), (i >> 1) & 1)) P.status[b] = 3;
+        if (t.x0 < 3 || by0 < 0 || t.x0 + kBtW + 3 > W || by0 + kBoxH > H) blur_reflect_box(box, bx0, by0, W, H);
+        blur_h_pass(box, s_h2);
         __syncthreads();
-    }
-    // horizontal pass: output x of box row py uses box bytes x + 13 .. x + 19 (image columns x0 + x - 3 .. + 3); for the
-    // outputs 4j .. 4j + 3 that is byte 1 of word j + 3 up to byte 2 of word j + 5
-    const uint32_t *src32 = reinterpret_cast<const uint32_t *>(s_src);
-    for (int i = tid; i < kBoxH * (kBtW / 4); i += 256) {
-        const int py = i >> 4, j = i & 15;
-        const uint32_t *w = src32 + py * (kBoxW / 4) + j + (kBoxX - 4) / 4;
-        const uint32_t A = w[0], B = w[1], C = w[2];
-        const uint32_t kW1 = 0x38302212u, kW2 = 0x00122230u;  // bytes (18, 34, 48, 56) and (48, 34, 18, 0)
-        const uint32_t h0 = __dp4a(__funnelshift_r(A, B, 8), kW1, __dp4a(__funnelshift_r(B, C, 8), kW2, 0u));
-        const uint32_t h1 = __dp4a(__funnelshift_r(A, B, 16), kW1, __dp4a(__funnelshift_r(B, C, 16), kW2, 0u));
-        const uint32_t h2 = __dp4a(__funnelshift_r(A, B, 24), kW1, __dp4a(__funnelshift_r(B, C, 24), kW2, 0u));
-        const uint32_t h3 = __dp4a(B, kW1, __dp4a(C, kW2, 0u));
-        *reinterpret_cast<uint2 *>(s_h + py * kBtW + 4 * j) = make_uint2(h0 | (h1 << 16), h2 | (h3 << 16));
-    }
-    __syncthreads();
-    uint8_t *dst = P.blur + (size_t)b * P.blur_frame_bytes + P.lv[l].blur_offset;
-    const int dpitch = P.lv[l].pitch;
-    for (int i = tid; i < kBtH * (kBtW / 4); i += 256) {
-        const int py = i >> 4, px = (i & 15) * 4;
-        if (t.y0 + py >= H || t.x0 + px >= W) continue;
-        uint2 r[7];
-#pragma unroll
-        for (int k = 0; k < 7; ++k) r[k] = *reinterpret_cast<const uint2 *>(s_h + (py + k) * kBtW + px);
-        uint32_t packed = 0;
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-            uint32_t h[7];
-#pragma unroll
-            for (int k = 0; k < 7; ++k) {
-                const uint32_t w = (c < 2) ? r[k].x : r[k].y;
-                h[k] = (c & 1) ? (w >> 16) : (w & 0xffffu);
-            }
-            const uint32_t acc = 18u * (h[0] + h[6]) + 34u * (h[1] + h[5]) + 48u * (h[2] + h[4]) + 56u * h[3];
-            packed |= ((acc + 32768u) >> 16) << (8 * c);
-        }
-        // pitch is a multiple of 64: aligned 4-byte store; bytes past the image width are padding
-        *reinterpret_cast<uint32_t *>(dst + (size_t)(t.y0 + py) * dpitch + t.x0 + px) = packed;
+        blur_v_pass(s_h2, P.blur + (size_t)b * P.blur_frame_bytes + P.lv[l].blur_offset, P.lv[l].pitch, t.x0, t.y0, W, H);
     }
 }
 
@@ -1745,7 +1807,7 @@ static plp_status orb_run(plp_orb *o, const uint8_t *d_imgs, int batch, size_t s
         PLP_LAUNCH(ctx, fast_cells_kernel_v2, grid, 256, 0, D);
     }
     if (D.num_blur_tiles > 0) {
-        dim3 grid(D.num_blur_tiles, batch);
+        dim3 grid(D.num_blur_tiles, batch), grid_run(div_up(D.num_blur_tiles, kBlurRun), batch);
         bool tma = o->maps_ok && !o->no_tma;
         if (tma && (o->map0_img != d_imgs || o->map0_step != step || o->map0_batch != batch)) {
             tma = encode_level_map(&o->maps.m[0], d_imgs, D.lv[0].w, D.lv[0].h, batch, step, D.img0_frame_stride);
@@ -1759,11 +1821,11 @@ static plp_status orb_run(plp_orb *o, const uint8_t *d_imgs, int batch, size_t s
                 PLP_CUDA_TRY(cudaMemcpyAsync(o->d_maps, &o->maps, sizeof(BlurMaps), cudaMemcpyHostToDevice, ctx->stream));
                 o->d_maps_dirty = false;
             }
-            PLP_LAUNCH(ctx, blur_tiles_tma_kernel<true>, grid, 256, 0, o->maps, o->d_maps, D);
+            PLP_LAUNCH(ctx, blur_tiles_tma_kernel<true>, grid_run, kBlurThreads, 0, o->maps, o->d_maps, D, kBlurRun);
         } else if (tma)
-            PLP_LAUNCH(ctx, blur_tiles_tma_kernel<false>, grid, 256, 0, o->maps, (const CUtensorMap *)nullptr, D);
+            PLP_LAUNCH(ctx, blur_tiles_tma_kernel<false>, grid_run, kBlurThreads, 0, o->maps, (const CUtensorMap *)nullptr, D, kBlurRun);
         else  // caller buffer not 16-byte aligned / pitched (or PLP_BLUR_NO_TMA=1 for A/B runs): plain loads
-            PLP_LAUNCH(ctx, blur_tiles_kernel, grid, 256, 0, D);
+            PLP_LAUNCH(ctx, blur_tiles_kernel, grid, kBlurThreads, 0, D);
     }
     {
         dim3 grid(D.num_levels, batch);
