@@ -307,6 +307,9 @@ PLP_API plp_status plp_orb_get_pyramid(const plp_orb *orb, int b, int level, plp
  * reference's cell order, coordinates relative to the 19-px border (orb_extractor.cc:424-434). */
 PLP_API plp_status plp_orb_debug_candidates(plp_orb *orb, int b, int level, plp_keypoint *out, int cap,
                                             int *n_out);
+/* The blurred level (cv::GaussianBlur 7x7, sigma 2, BORDER_REFLECT_101) the descriptors of frame b of the most recent
+ * extraction sample, copied densely into out (rows x cols of that level, as plp_orb_get_pyramid reports them). */
+PLP_API plp_status plp_orb_debug_blurred(plp_orb *orb, int b, int level, uint8_t *out);
 
 /* robust::match_for_triangulation (match/robust.cc:43-216): for every landmark-free keypoint of keyframe 1 (visited in
  * the order of its BoW feature vector: ascending node id, then the node's index list) the landmark-free, not yet taken

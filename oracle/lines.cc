@@ -341,17 +341,26 @@ constexpr unsigned kBins = 1024;
 void scaled_image(const uint8_t *img, int w, int h, int step, std::vector<uint8_t> &out, int &sw, int &sh) {
     std::vector<uint8_t> g((size_t)w * h);
     blur_q8(img, w, h, step, g.data(), w, kGauss11, 11);
-    // resize(..., Size(), 0.5, 0.5, INTER_LINEAR_EXACT): dsize = round(w * 0.5); at exactly 1/2 every destination pixel is
-    // the rounded mean of a 2x2 block (fixed point, ties up)
+    // resize(..., Size(), 0.5, 0.5, INTER_LINEAR_EXACT): dsize = round(w * 0.5), ties to even, so a dimension n = 3 (mod 4)
+    // gets a last destination row / column with one source row / column (n = 1 (mod 4) drops the last source one).
+    // At exactly 1/2 cv2 resizes by area over the source pixels that exist (derived from cv2 4.13 with impulses,
+    // exhaustive value pairs in the last row and column and the corner, see test_lines_oracle.py):
+    //   full 2x2 block:                          (s + 2) >> 2            (fixed point, ties up)
+    //   last row or column, 2 source pixels:     s / 2, ties to even     (float sum / count, cvRound)
+    //   corner, 1 source pixel:                  the pixel
     sw = (int)std::lrint(w * kScale);
     sh = (int)std::lrint(h * kScale);
     out.assign((size_t)sw * sh, 0);
     for (int y = 0; y < sh; ++y)
         for (int x = 0; x < sw; ++x) {
-            const int x0 = std::min(2 * x, w - 1), x1 = std::min(2 * x + 1, w - 1);
-            const int y0 = std::min(2 * y, h - 1), y1 = std::min(2 * y + 1, h - 1);
-            const int s = g[(size_t)y0 * w + x0] + g[(size_t)y0 * w + x1] + g[(size_t)y1 * w + x0] + g[(size_t)y1 * w + x1];
-            out[(size_t)y * sw + x] = (uint8_t)((s + 2) >> 2);
+            const int x0 = 2 * x, x1 = std::min(2 * x + 1, w - 1);
+            const int y0 = 2 * y, y1 = std::min(2 * y + 1, h - 1);
+            int s = g[(size_t)y0 * w + x0];
+            if (x1 != x0) s += g[(size_t)y0 * w + x1];
+            if (y1 != y0) s += g[(size_t)y1 * w + x0];
+            if (x1 != x0 && y1 != y0) s += g[(size_t)y1 * w + x1];
+            const int n = (x1 != x0 ? 2 : 1) * (y1 != y0 ? 2 : 1);
+            out[(size_t)y * sw + x] = (uint8_t)(n == 4 ? (s + 2) >> 2 : n == 2 ? (s + ((s >> 1) & 1)) >> 1 : s);
         }
 }
 

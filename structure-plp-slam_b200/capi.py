@@ -765,6 +765,14 @@ class OrbExtractor:
                                                             out.ctypes.data_as(_P), C.c_int(cap), C.byref(n)))
         return out[:min(n.value, cap)].copy()
 
+    def debug_blurred(self, b: int, level: int) -> np.ndarray:
+        """The blurred level the descriptors of frame b of the last extraction sample (downloaded)."""
+        v = ImageView()
+        self._ctx._check(self._lib.plp_orb_get_pyramid(self._h, C.c_int(b), C.c_int(level), C.byref(v)))
+        out = np.zeros((v.rows, v.cols), np.uint8)
+        self._ctx._check(self._lib.plp_orb_debug_blurred(self._h, C.c_int(b), C.c_int(level), out.ctypes.data_as(_P)))
+        return out
+
 
 # binary layout of plp_keyline / cv::line_descriptor::KeyLine (descriptor_custom.hpp:105-199)
 KEYLINE_DTYPE = np.dtype([("angle", "<f4"), ("class_id", "<i4"), ("octave", "<i4"), ("pt_x", "<f4"), ("pt_y", "<f4"),

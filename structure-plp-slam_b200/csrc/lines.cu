@@ -42,7 +42,8 @@ __device__ __forceinline__ int reflect101(int p, int len) {
 
 // ------------------------------------------------------------------------------------------------------------------
 // K1: GaussianBlur(11x11, sigma 1.2) in OpenCV's Q8 fixed point (taps 0 0 4 21 60 86 60 21 4 0 0) followed by
-//     resize(0.5, INTER_LINEAR_EXACT) == rounded mean of each 2x2 block.  One CTA = 64 x 16 source pixels.
+//     resize(0.5, INTER_LINEAR_EXACT) == rounded mean of each 2x2 block (of its existing pixels at an odd border).
+//     One CTA = 64 x 16 source pixels.
 // ------------------------------------------------------------------------------------------------------------------
 constexpr int kScTw = 64, kScTh = 16;
 __global__ void __launch_bounds__(256) lsd_scale_kernel(LineDev D) {
@@ -77,11 +78,20 @@ __global__ void __launch_bounds__(256) lsd_scale_kernel(LineDev D) {
         const int r = i / (kScTw / 2), c = i - r * (kScTw / 2);
         const int ox = tx / 2 + c, oy = ty / 2 + r;
         if (ox >= D.sw || oy >= D.sh) continue;
-        // clamp like the oracle for odd sizes (min(2x+1, w-1)); inside the tile the clamped pixel is the same column/row
-        const int x0 = 2 * c, x1 = (tx + 2 * c + 1 < D.w) ? 2 * c + 1 : 2 * c;
-        const int y0 = 2 * r, y1 = (ty + 2 * r + 1 < D.h) ? 2 * r + 1 : 2 * r;
-        const int s = s_b[y0][x0] + s_b[y0][x1] + s_b[y1][x0] + s_b[y1][x1];
-        out[(size_t)oy * D.sw + ox] = (uint8_t)((s + 2) >> 2);
+        // a dimension = 3 (mod 4) has a last half-resolution row / column with one source row / column: cv2 averages
+        // the pixels that exist there, s / 2 ties to even, and copies the corner (the oracle's scaled_image states it)
+        const bool fx = tx + 2 * c + 1 < D.w, fy = ty + 2 * r + 1 < D.h;
+        const int x0 = 2 * c, y0 = 2 * r;
+        int v;
+        if (fx && fy) {
+            v = (s_b[y0][x0] + s_b[y0][x0 + 1] + s_b[y0 + 1][x0] + s_b[y0 + 1][x0 + 1] + 2) >> 2;
+        } else if (fx || fy) {
+            const int s = s_b[y0][x0] + (fx ? s_b[y0][x0 + 1] : s_b[y0 + 1][x0]);
+            v = (s + ((s >> 1) & 1)) >> 1;
+        } else {
+            v = s_b[y0][x0];
+        }
+        out[(size_t)oy * D.sw + ox] = (uint8_t)v;
     }
 }
 

@@ -1829,7 +1829,8 @@ static plp_status orb_run(plp_orb *o, const uint8_t *d_imgs, int batch, size_t s
     }
     {
         dim3 grid(D.num_levels, batch);
-        if (ctx->timing) plp::timing_begin(ctx, "quadtree_kernel");  // (PLP_LAUNCH spelled out: one name for both instances)
+        // (PLP_LAUNCH spelled out: the report names the instance by its node capacity)
+        if (ctx->timing) plp::timing_begin(ctx, o->qt_small ? "quadtree_kernel<1024>" : "quadtree_kernel<2048>");
         if (o->qt_small)
             quadtree_kernel<kNodeCapSmall, kCandCapSmall, 2><<<grid, kQtThreads, o->qt_smem, ctx->stream>>>(D);
         else
@@ -1919,6 +1920,18 @@ plp_status plp_orb_get_pyramid(const plp_orb *o, int b, int level, plp_image_vie
         out->data = o->d_pyr + (size_t)b * o->dev.pyr_frame_bytes + V.offset;
         out->step = V.pitch;
     }
+    return PLP_OK;
+}
+
+plp_status plp_orb_debug_blurred(plp_orb *o, int b, int level, uint8_t *out) {
+    PLP_REQUIRE(o && out, "null pointer");
+    PLP_REQUIRE(b >= 0 && b < o->last_batch && level >= 0 && level < o->dev.num_levels, "index");
+    plp_ctx *ctx = o->ctx;
+    PLP_CUDA_TRY(cudaSetDevice(ctx->device));
+    const LevelInfo &V = o->dev.lv[level];
+    PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
+    PLP_CUDA_TRY(cudaMemcpy2D(out, V.w, o->d_blur + (size_t)b * o->dev.blur_frame_bytes + V.blur_offset, V.pitch, V.w, V.h,
+                              cudaMemcpyDeviceToHost));
     return PLP_OK;
 }
 

@@ -1,7 +1,8 @@
 // stereo.cu -- match::stereo::compute (match/stereo.cc:45-302) for batches of rectified stereo frames, sm_90a.
 //
 // One CTA per frame.  The right keypoints (row band, x, octave, 256-bit descriptor) are staged in shared memory once;
-// a warp owns one left keypoint at a time: lanes scan the right keypoints in ascending index order (the order of the
+// when the descriptors do not fit (capacity above ~5100, i.e. max_num_keypts 2000 as in the KITTI stereo configs) they
+// are read from global memory (L2) instead, with the same comparisons.  A warp owns one left keypoint at a time: lanes scan the right keypoints in ascending index order (the order of the
 // reference's per-row candidate lists), the 256-bit Hamming distance is 8 x __popc, and the warp minimum of
 // (distance << 16 | index) is exactly the reference's "first strictly smaller distance wins".  The 11 x 11 L1 patch
 // slide (11 offsets) reads the image pyramids the two ORB handles keep in HBM (orb_extractor::image_pyramid_,
@@ -38,11 +39,11 @@ struct StereoDev {
     int32_t *best_right;  // optional parity tap
 };
 
+template <bool kDescSmem>
 __global__ void __launch_bounds__(kThreads, 1) stereo_kernel(StereoDev D) {
     extern __shared__ uint4 s_dyn[];
-    // layout: desc_r [cap][2 x uint4] | band [cap] short2 | xr [cap] float | oct [cap] int8 | corr [cap] int
-    uint4 *s_desc = s_dyn;
-    short2 *s_band = reinterpret_cast<short2 *>(s_desc + 2 * (size_t)D.cap);
+    // layout: [desc_r [cap][2 x uint4] if kDescSmem] | band [cap] short2 | xr [cap] float | corr [cap] int | oct [cap] int8
+    short2 *s_band = reinterpret_cast<short2 *>(s_dyn + (kDescSmem ? 2 * (size_t)D.cap : 0));
     float *s_x = reinterpret_cast<float *>(s_band + D.cap);
     int *s_corr = reinterpret_cast<int *>(s_x + D.cap);
     int8_t *s_oct = reinterpret_cast<int8_t *>(s_corr + D.cap);
@@ -52,6 +53,7 @@ __global__ void __launch_bounds__(kThreads, 1) stereo_kernel(StereoDev D) {
     const plp_keypoint *kpl = D.kp_l + (size_t)b * D.cap, *kpr = D.kp_r + (size_t)b * D.cap;
     const uint4 *dl = reinterpret_cast<const uint4 *>(D.desc_l + (size_t)b * D.cap * 32);
     const uint4 *dr = reinterpret_cast<const uint4 *>(D.desc_r + (size_t)b * D.cap * 32);
+    const uint4 *s_desc = kDescSmem ? s_dyn : dr;
     float *xr_out = D.x_right + (size_t)b * D.cap, *dp_out = D.depth + (size_t)b * D.cap;
     for (int i = tid; i < nr; i += kThreads) {
         const plp_keypoint k = kpr[i];
@@ -59,8 +61,10 @@ __global__ void __launch_bounds__(kThreads, 1) stereo_kernel(StereoDev D) {
         s_band[i] = make_short2((short)cv_floor((double)(k.y - r)), (short)cv_ceil((double)(k.y + r)));
         s_x[i] = k.x;
         s_oct[i] = (int8_t)k.octave;
-        s_desc[2 * i] = dr[2 * i];
-        s_desc[2 * i + 1] = dr[2 * i + 1];
+        if (kDescSmem) {
+            s_dyn[2 * i] = dr[2 * i];
+            s_dyn[2 * i + 1] = dr[2 * i + 1];
+        }
     }
     for (int i = tid; i < nl; i += kThreads) {
         s_corr[i] = -1;
@@ -185,7 +189,7 @@ __global__ void __launch_bounds__(kThreads, 1) stereo_kernel(StereoDev D) {
     }
 }
 
-size_t stereo_smem(int cap) { return (size_t)cap * (32 + 4 + 4 + 4 + 1) + 16; }
+size_t stereo_smem(int cap, bool desc_smem) { return (size_t)cap * ((desc_smem ? 32 : 0) + 4 + 4 + 4 + 1) + 16; }
 
 plp_status fill_levels(const plp_orb *left, const plp_orb *right, int batch, StereoDev &D) {
     for (int l = 0; l < D.num_levels; ++l) {
@@ -254,9 +258,17 @@ plp_status plp_stereo_compute_batch_dev(plp_ctx *ctx, const plp_orb *left, const
     D.x_right = d_x_right_out;
     D.depth = d_depth_out;
     D.best_right = d_best_right_out;
-    const size_t smem = stereo_smem(D.cap);
-    PLP_SMEM_OPTIN(stereo_kernel, smem);
-    PLP_LAUNCH(ctx, stereo_kernel, batch, kThreads, smem, D);
+    int optin = 0;
+    PLP_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, ctx->device));
+    if (stereo_smem(D.cap, true) + 64 <= (size_t)optin) {  // (+ the static shared words)
+        const size_t smem = stereo_smem(D.cap, true);
+        PLP_SMEM_OPTIN(stereo_kernel<true>, smem);
+        PLP_LAUNCH(ctx, stereo_kernel<true>, batch, kThreads, smem, D);
+    } else {
+        const size_t smem = stereo_smem(D.cap, false);
+        PLP_SMEM_OPTIN(stereo_kernel<false>, smem);
+        PLP_LAUNCH(ctx, stereo_kernel<false>, batch, kThreads, smem, D);
+    }
     PLP_CHECK_LAUNCH();
     return PLP_OK;
 }

@@ -57,6 +57,11 @@ class PlanarSequence:
                                                    borderMode=cv2.BORDER_REFLECT_101))
         self.frames = np.stack(self.frames)
 
+    def camera(self, plp):
+        """The plp_camera of K at this sequence's size."""
+        K = self.K
+        return plp.capi.make_camera(K[0, 0], K[1, 1], K[0, 2], K[1, 2], self.cols, self.rows)
+
     def _KM(self, T):
         R, t = T[:3, :3], T[:3, 3]
         M = np.stack([R[:, 0], R[:, 1], R[:, 2] * Z0 + t], 1)
@@ -90,11 +95,11 @@ class PlanarSequence:
 def oracle_track(orc, plp, seq, res, t, T_pred, margin=20.0):
     """The oracle chain of frame_tracker::motion_based_track for frame t of `seq`: match_current_and_last_frames
     (retried with 2 x margin below 20 matches) -> pose_optimize -> discard_outliers.  res[t - 1] / res[t] are oracle
-    ORB extractions; plp is the package (only its ctypes structures are used).
+    ORB extractions; plp is the package (only its ctypes structures are used).  The camera is the sequence's own (K).
     Returns (matched, pose, num_valid, n_inliers, LM iterations)."""
     import oracle_api
     grid = plp.capi.make_grid(seq.cols, seq.rows)
-    cam = plp.capi.make_camera(synth.FX, synth.FY, synth.CX, synth.CY, seq.cols, seq.rows)
+    cam = seq.camera(plp)
     sf, isig = synth.scale_factors(), synth.inv_level_sigma_sq()
     last = seq.last_frame_landmarks(t - 1, res[t - 1]["kps"], res[t - 1]["desc"])
     k = res[t]["kps"]

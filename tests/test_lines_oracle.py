@@ -7,6 +7,7 @@
 * LBD itself is vendored reference source (binary_descriptor_custom.cpp) restated line by line: structural checks.
 * detmath (deterministic sin/cos/atan2) against libm, and the two textual copies are identical.
 """
+import functools
 import math
 from pathlib import Path
 
@@ -18,6 +19,13 @@ import synth
 
 cv2 = pytest.importorskip("cv2")
 ROOT = Path(__file__).resolve().parent.parent
+
+
+# camera geometries the reference ships (KITTI 00-02 1241 x 376, KITTI 03 1242 x 375, KITTI 04-12 1226 x 370, TUM-VI
+# 512 x 512) and sizes that, with the rest, cover every residue mod 4 of rows and of cols: a dimension = 3 (mod 4) gives the
+# half-resolution image a last row / column with a single source row / column
+GEOMETRIES = [(375, 1242), (370, 1226), (376, 1241), (512, 512), (479, 639), (481, 641), (478, 637), (33, 47), (47, 33),
+              (16, 16)] + [(64 + r, 96 + c) for r in range(4) for c in range(4)]
 
 
 def _images():
@@ -32,17 +40,83 @@ def _images():
     return out
 
 
+GEOMETRY_NAMES = [f"{'texture' if i % 2 == 0 else 'lines'}{h}x{w}" for i, (h, w) in enumerate(GEOMETRIES)]
+
+
+@functools.lru_cache(maxsize=1)
+def _geometry_images():
+    """One seeded image per GEOMETRIES entry, textures and line images alternating."""
+    return {n: synth.make_texture(40 + i, h, w) if i % 2 == 0 else synth.make_line_image(40 + i, h, w)
+            for i, (n, (h, w)) in enumerate(zip(GEOMETRY_NAMES, GEOMETRIES))}
+
+
 def _cv_lsd(img):
     lsd = cv2.createLineSegmentDetector(1, 0.5, 0.6, 2.0, 22.5, 1.0, 0.6, 1024)
     r = lsd.detect(img)[0]
     return np.zeros((0, 4), np.float32) if r is None else r.reshape(-1, 4)
 
 
+def half_area(g):
+    """resize(g, None, 0.5, 0.5, INTER_LINEAR_EXACT) as oracle/lines.cc states it: the mean of each 2x2 block's existing
+    pixels -- 4 pixels (s + 2) >> 2, 2 pixels (last row or column of a dimension = 3 mod 4) s / 2 ties to even, 1 pixel
+    (that corner) the pixel."""
+    h, w = g.shape
+    sh, sw = int(np.rint(h * 0.5)), int(np.rint(w * 0.5))
+    gi = np.zeros((2 * sh, 2 * sw), np.int64)
+    n = np.zeros_like(gi)
+    hh, ww = min(h, 2 * sh), min(w, 2 * sw)
+    gi[:hh, :ww] = g[:hh, :ww]
+    n[:hh, :ww] = 1
+    s = gi.reshape(sh, 2, sw, 2).sum((1, 3))
+    c = n.reshape(sh, 2, sw, 2).sum((1, 3))
+    return np.where(c == 4, (s + 2) >> 2, np.where(c == 2, (s + ((s >> 1) & 1)) >> 1, s)).astype(np.uint8)
+
+
+def test_half_resize_border_rule_is_cv2s():
+    """The border rule of half_area derived from cv2 itself: every value pair in a 2-pixel last column and last row, every
+    value of the 1-pixel corner, impulses (each source pixel feeds only its own block, or nothing) and seeded images at
+    every residue mod 4."""
+    def cvr(img):
+        return cv2.resize(img, None, fx=0.5, fy=0.5, interpolation=cv2.INTER_LINEAR_EXACT)
+    a, b = np.meshgrid(np.arange(256), np.arange(256), indexing="ij")
+    col = np.zeros((2 * 256 * 256, 7), np.uint8)            # 7 cols -> 4, last column from col 6 only
+    col[0::2, 6], col[1::2, 6] = a.ravel(), b.ravel()
+    assert np.array_equal(cvr(col)[:, 3].astype(np.int64), ((a + b) + (((a + b) >> 1) & 1)).ravel() >> 1)
+    row = np.zeros((7, 2 * 256 * 256), np.uint8)
+    row[6, 0::2], row[6, 1::2] = a.ravel(), b.ravel()
+    assert np.array_equal(cvr(row)[3].astype(np.int64), ((a + b) + (((a + b) >> 1) & 1)).ravel() >> 1)
+    corner = np.zeros((256, 7, 7), np.uint8)                # 7 x 7 -> 4 x 4, corner from pixel (6, 6) only
+    corner[:, 6, 6] = np.arange(256)
+    assert [int(cvr(c)[3, 3]) for c in corner] == list(range(256))
+    for h, w in ((7, 7), (11, 15), (9, 13)):
+        for y in range(h):
+            for x in range(w):
+                img = np.zeros((h, w), np.uint8)
+                img[y, x] = 201
+                r = cvr(img)
+                # a dimension = 1 (mod 4) drops its last source row / column
+                inside = y // 2 < r.shape[0] and x // 2 < r.shape[1]
+                assert np.array_equal(np.argwhere(r), [[y // 2, x // 2]] if inside else np.zeros((0, 2)))
+    rng = np.random.default_rng(0)
+    for h in range(16, 24):
+        for w in range(16, 24):
+            g = rng.integers(0, 256, (h, w), dtype=np.uint8)
+            assert np.array_equal(cvr(g), half_area(g)), (h, w)
+
+
+def _cv_scaled(img):
+    g = cv2.GaussianBlur(img, (11, 11), 1.2)
+    return cv2.resize(g, None, fx=0.5, fy=0.5, interpolation=cv2.INTER_LINEAR_EXACT)
+
+
+def _cv_lbd_gradients(img):
+    g = cv2.GaussianBlur(img, (5, 5), 1)
+    return cv2.Sobel(g, cv2.CV_16S, 1, 0, ksize=3), cv2.Sobel(g, cv2.CV_16S, 0, 1, ksize=3)
+
+
 def test_scaled_image_matches_cv2(orc):
     for name, img in _images():
-        g = cv2.GaussianBlur(img, (11, 11), 1.2)
-        s = cv2.resize(g, None, fx=0.5, fy=0.5, interpolation=cv2.INTER_LINEAR_EXACT)
-        assert np.array_equal(orc.lsd_scaled(img), s), name
+        assert np.array_equal(orc.lsd_scaled(img), _cv_scaled(img)), name
 
 
 @pytest.mark.parametrize("mode", [oracle_api.LSD_DET, oracle_api.LSD_CV])
@@ -59,11 +133,36 @@ def test_lsd_segments_bit_exact_vs_cv2(orc, mode):
 
 def test_lbd_gradients_match_cv2(orc):
     for name, img in _images()[:5]:
-        g = cv2.GaussianBlur(img, (5, 5), 1)
-        dx = cv2.Sobel(g, cv2.CV_16S, 1, 0, ksize=3)
-        dy = cv2.Sobel(g, cv2.CV_16S, 0, 1, ksize=3)
+        dx, dy = _cv_lbd_gradients(img)
         ox, oy = orc.lbd_gradients(img)
         assert np.array_equal(ox, dx) and np.array_equal(oy, dy), name
+
+
+# the same three comparisons at the camera geometries and at every residue mod 4, one case per size
+@pytest.mark.parametrize("name", GEOMETRY_NAMES)
+def test_scaled_image_matches_cv2_at_size(orc, name):
+    img = _geometry_images()[name]
+    assert np.array_equal(orc.lsd_scaled(img), _cv_scaled(img)), name
+
+
+@pytest.mark.parametrize("mode", [oracle_api.LSD_DET, oracle_api.LSD_CV])
+@pytest.mark.parametrize("name", GEOMETRY_NAMES)
+def test_lsd_segments_bit_exact_vs_cv2_at_size(orc, mode, name):
+    img = _geometry_images()[name]
+    ref = _cv_lsd(img)
+    got = orc.lsd_detect(img, mode)
+    assert got.shape == ref.shape, f"{name}: {len(got)} vs {len(ref)} segments"
+    assert np.array_equal(got, ref), name
+    if min(img.shape) >= 64:
+        assert len(ref) > 0
+
+
+@pytest.mark.parametrize("name", GEOMETRY_NAMES)
+def test_lbd_gradients_match_cv2_at_size(orc, name):
+    img = _geometry_images()[name]
+    dx, dy = _cv_lbd_gradients(img)
+    ox, oy = orc.lbd_gradients(img)
+    assert np.array_equal(ox, dx) and np.array_equal(oy, dy), name
 
 
 def test_keyline_fields_and_line_iterator_count(orc):

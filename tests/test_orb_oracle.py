@@ -209,7 +209,26 @@ def _cv2_mirror_extract(orc, p, img):
             kl["x"] = (kl["x"] * s).astype(np.float32)
             kl["y"] = (kl["y"] * s).astype(np.float32)
         kps_all.append(kl)
-    return np.concatenate(kps_all), np.array(desc_all, np.uint8), pyr
+    # a small image can leave every level without a keypoint
+    kps = np.concatenate(kps_all) if kps_all else np.zeros(0, oracle_api.KP_DTYPE)
+    return kps, np.array(desc_all, np.uint8).reshape(-1, 32), pyr
+
+
+@pytest.mark.parametrize("shape", [(40, 41), (41, 40), (48, 64), (75, 100), (120, 160)])
+def test_small_images_match_cv2_mirror(orc, shape):
+    """Upper levels of a small image have no FAST cell (w or h <= 38); 41 x 40 has no keypoint at any level."""
+    img = synth.make_texture(9, *shape)
+    p = oracle_api.orb_params()
+    r = orc.orb_extract(p, img)
+    kps, desc, pyr = _cv2_mirror_extract(orc, p, img)
+    for a, b in zip(pyr, r["pyramid"]):
+        assert np.array_equal(a, b)
+    assert len(kps) == len(r["kps"]) and desc.shape == r["desc"].shape
+    for f in ("x", "y", "size", "angle", "response", "octave"):
+        assert np.array_equal(kps[f], r["kps"][f]), f
+    assert np.array_equal(desc, r["desc"])
+    if min(shape) >= 75:
+        assert len(kps) > 10
 
 
 @pytest.mark.parametrize("seed,shape", [(1234, (480, 640)), (77, (480, 752))])

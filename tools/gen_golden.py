@@ -7,7 +7,10 @@ cv2_primitives.npz  cv::resize / cv::FAST / cv::GaussianBlur 7x7 + 5x5 / cv::Sob
 cv2_lsd.npz         cv::LineSegmentDetector(1, 0.5, 0.6, 2, 22.5, 1, 0.6, 1024) segments on two seeded images
 orb_mirror.npz      orb_extractor::extract with every third-party stage done by cv2 (tests/test_orb_oracle.py mirror)
 line_extract.npz    LineFeatureTracker::extract_LSD_LBD output of the oracle (whose LSD stage is pinned to cv2 above)
-The images are regenerated from their seeds by the tests; only the outputs are stored."""
+cv2_lsd_odd.npz     cv2's half-resolution LSD image and LSD segments at sizes with a dimension = 3 (mod 4)
+The images are regenerated from their seeds by the tests; only the outputs are stored.
+
+    python tools/gen_golden.py cv2_lsd_odd      # only the named files"""
 import sys
 from pathlib import Path
 
@@ -18,13 +21,30 @@ ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT / "tests"))
 import oracle_api  # noqa: E402
 import synth  # noqa: E402
+import test_golden  # noqa: E402
 import test_orb_oracle  # noqa: E402
 
 OUT = ROOT / "tests" / "golden"
 
 
+def lsd_odd():
+    lsd = cv2.createLineSegmentDetector(1, 0.5, 0.6, 2.0, 22.5, 1.0, 0.6, 1024)
+    out = {}
+    for kind, seed, h, w in test_golden.LSD_ODD:
+        img, key = test_golden.lsd_odd_image(kind, seed, h, w), f"{kind}_{seed}"
+        g = cv2.GaussianBlur(img, (11, 11), 1.2)
+        out[key + "_scaled"] = cv2.resize(g, None, fx=0.5, fy=0.5, interpolation=cv2.INTER_LINEAR_EXACT)
+        r = lsd.detect(img)[0]
+        out[key] = np.zeros((0, 4), np.float32) if r is None else r.reshape(-1, 4)
+    np.savez_compressed(OUT / "cv2_lsd_odd.npz", **out)
+
+
 def main():
     OUT.mkdir(exist_ok=True)
+    if sys.argv[1:]:
+        for name in sys.argv[1:]:
+            {"cv2_lsd_odd": lsd_odd}[name]()
+        return
     orc = oracle_api.Oracle()
     tex = synth.make_texture(4321, 240, 320, n_rect=120, n_blob=500)      # the image of __graft_entry__.smoke()
     lines = synth.make_line_image(7, 240, 320, n_patch=16)
@@ -59,6 +79,7 @@ def main():
     # ---- line extraction (oracle, LSD pinned to cv2)
     kl, lbd, fn = orc.line_extract(lines)
     np.savez_compressed(OUT / "line_extract.npz", keylines=kl, lbd=lbd, line_functions=fn)
+    lsd_odd()
     for f in sorted(OUT.glob("*.npz")):
         print(f.name, f.stat().st_size, "bytes")
 
