@@ -140,6 +140,14 @@ typedef struct plp_camera {
     int32_t setup_type;               /* 0 Monocular, 1 Stereo, 2 RGBD (camera/base.h setup_type_t) */
 } plp_camera;
 
+typedef struct plp_distortion {
+    /* Camera.model and its coefficients as the config gives them (the library rounds them to float, as the reference's
+     * cv::Mat_<float> does): model 0 perspective, k = (k1, k2, p1, p2, k3); model 1 fisheye, k = (k1, k2, k3, k4, -). */
+    int32_t model;
+    double k[5];
+} plp_distortion;
+
+
 /* ------------------------------------------------------------------------ */
 /* projection matchers (match/projection.cc)                                 */
 /* ------------------------------------------------------------------------ */
@@ -263,6 +271,22 @@ typedef struct plp_keypoint { /* binary layout of cv::KeyPoint (28 bytes) */
     float size, angle, response;
     int32_t octave, class_id;
 } plp_keypoint;
+
+/* camera::{perspective,fisheye}::compute_image_bounds (perspective.cc:100-127, fisheye.cc:101-169) of cam's fx, fy, cx, cy
+ * (host computation): bounds_out = (min_x, max_x, min_y, max_y), the img_bounds_ of plp_camera and of the grid. */
+PLP_API plp_status plp_camera_image_bounds(const plp_camera *cam, const plp_distortion *dist, int cols, int rows,
+                                           float bounds_out[4]);
+/* undistort_keypoints + convert_keypoints_to_bearings (perspective.cc:130-175, fisheye.cc:172-215).  Host pointers.
+ * undist_out[i] = kp[i] with pt undistorted (cv::undistortPoints / cv::fisheye::undistortPoints); angle, size and octave
+ * copied, response 0, class_id -1.  bearings_out (n x 3) may be NULL.  n == 0 -> PLP_OK. */
+PLP_API plp_status plp_undistort_keypoints(plp_ctx *ctx, const plp_camera *cam, const plp_distortion *dist,
+                                           const plp_keypoint *kp, int n, plp_keypoint *undist_out, double *bearings_out);
+/* Device-resident batched form for the layout plp_orb_extract_batch_dev writes: frame b owns d_kp[b * cap ..] with
+ * d_n_kp[b] keypoints.  Writes d_undist_out (batch x cap) and, when not NULL, d_bearings_out (batch x cap x 3); slots past
+ * a frame's count are left untouched.  No synchronisation. */
+PLP_API plp_status plp_undistort_keypoints_batch_dev(plp_ctx *ctx, const plp_camera *cam, const plp_distortion *dist,
+                                                     int batch, int cap, const plp_keypoint *d_kp, const int32_t *d_n_kp,
+                                                     plp_keypoint *d_undist_out, double *d_bearings_out);
 
 typedef struct plp_image_view { /* one pyramid level, device memory */
     const uint8_t *data;
@@ -684,6 +708,20 @@ PLP_API plp_status plp_tracker_create(plp_ctx *ctx, const plp_camera *cam, const
                                       const float *scale_factors, const float *inv_level_sigma_sq,
                                       int num_levels, int max_batch, int kp_capacity, int max_last_points,
                                       plp_tracker **out);
+/* A tracker for a distorted camera (frame.cc:68-86): motion_track_batch_dev first undistorts the current frames'
+ * keypoints (plp_undistort_keypoints_batch_dev into tracker-owned arrays), and the grid, the window queries and the pose
+ * optimiser's observations use the undistorted coordinates.  cam's min/max and grid must be built from
+ * plp_camera_image_bounds.  dist == NULL or a perspective model with all coefficients 0 is plp_tracker_create: no extra
+ * launch, the same outputs. */
+PLP_API plp_status plp_tracker_create_ex(plp_ctx *ctx, const plp_camera *cam, const plp_grid *grid,
+                                         const float *scale_factors, const float *inv_level_sigma_sq,
+                                         int num_levels, int max_batch, int kp_capacity, int max_last_points,
+                                         const plp_distortion *dist, plp_tracker **out);
+/* The undistorted keypoints (max_batch x kp_capacity) and bearings (x 3) of the most recent motion_track_batch_dev of a
+ * distorted tracker: device pointers owned by the tracker, valid once its stream has reached that call.  A tracker
+ * without distortion has none (PLP_ERR_INVALID): its undistorted keypoints are the ORB keypoints. */
+PLP_API plp_status plp_tracker_undistorted(const plp_tracker *t, const plp_keypoint **d_undist_kp,
+                                           const double **d_bearings);
 PLP_API void plp_tracker_destroy(plp_tracker *t);
 /* d_kp/d_desc/d_n_kp: the arrays written by plp_orb_extract_batch_dev (batch x kp_capacity entries).
  * Outputs (device): matched_out[batch x kp_capacity] = last-frame landmark index kept on each keypoint after

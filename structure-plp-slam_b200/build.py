@@ -35,6 +35,7 @@ FILE_FLAGS = {
     "bow.cu": NO_FMA,
     "essential.cu": NO_FMA,
     "plane.cu": NO_FMA,
+    "camera.cu": NO_FMA,
 }
 
 

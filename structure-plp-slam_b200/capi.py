@@ -62,6 +62,13 @@ class Camera(C.Structure):
 _P = C.c_void_p
 
 
+class Distortion(C.Structure):
+    _fields_ = [("model", C.c_int32), ("k", C.c_double * 5)]
+
+
+PERSPECTIVE, FISHEYE = 0, 1
+
+
 class FramePoints(C.Structure):
     _fields_ = [("n", C.c_int32), ("x", _P), ("y", _P), ("octave", _P), ("angle", _P), ("x_right", _P),
                 ("desc", _P), ("claimed", _P)]
@@ -196,6 +203,33 @@ def make_camera(fx, fy, cx, cy, cols, rows, bf=-1.0, setup_type=0) -> Camera:
     return Camera(fx, fy, cx, cy, bf, (bf / fx) if bf > 0 else -1.0, 0.0, float(cols), 0.0, float(rows), setup_type)
 
 
+def make_distortion(model, *k) -> Distortion:
+    """plp_distortion of a config: model 0 perspective (k1, k2, p1, p2, k3) or 1 fisheye (k1, k2, k3, k4); the
+    coefficients as the YAML gives them (the library rounds them to float like the reference)."""
+    if model not in (PERSPECTIVE, FISHEYE) or len(k) > (5 if model == PERSPECTIVE else 4):
+        raise PlpError(f"distortion model {model} with {len(k)} coefficients")
+    return Distortion(model, (C.c_double * 5)(*([float(v) for v in k] + [0.0] * (5 - len(k)))))
+
+
+def image_bounds(cam: Camera, dist: Distortion, cols: int, rows: int) -> np.ndarray:
+    """camera::*::compute_image_bounds through plp_camera_image_bounds -> float32 (min_x, max_x, min_y, max_y)."""
+    out = np.zeros(4, np.float32)
+    st = lib().plp_camera_image_bounds(C.byref(cam), C.byref(dist), C.c_int(cols), C.c_int(rows), out.ctypes.data_as(_P))
+    if st != 0:
+        raise PlpError(f"plp status {st}: {lib().plp_last_error().decode()}")
+    return out
+
+
+def make_distorted_camera(fx, fy, cx, cy, cols, rows, dist: Distortion, num_cols: int = 64, num_rows: int = 48):
+    """(plp_camera, plp_grid) of a distorted camera: img_bounds_ and the grid from the undistorted image corners, as the
+    camera::perspective / camera::fisheye constructors compute them."""
+    cam = make_camera(fx, fy, cx, cy, cols, rows)
+    b = image_bounds(cam, dist, cols, rows)
+    cam.min_x, cam.max_x, cam.min_y, cam.max_y = (float(v) for v in b)
+    grid = make_grid(cols, rows, num_cols, num_rows, min_x=b[0], min_y=b[2], max_x=b[1], max_y=b[3])
+    return cam, grid
+
+
 class Context:
     """One plp_ctx (device + stream).  Methods are named after the reference methods they replace."""
 
@@ -235,6 +269,21 @@ class Context:
 
     def launch_count(self) -> int:
         return int(self._lib.plp_ctx_launch_count(self._h))
+
+    # ------------------------------------------------------------------ camera::{perspective,fisheye}
+    def undistort_keypoints(self, cam, dist, kps):
+        """undistort_keypoints + convert_keypoints_to_bearings of a host KP_DTYPE array -> (undistorted kps, bearings)."""
+        kp = np.ascontiguousarray(kps, KP_DTYPE)
+        out = np.zeros(len(kp), KP_DTYPE)
+        bear = np.zeros((len(kp), 3), np.float64)
+        self._check(self._lib.plp_undistort_keypoints(self._h, C.byref(cam), C.byref(dist), kp.ctypes.data_as(_P),
+                                                      C.c_int(len(kp)), out.ctypes.data_as(_P), bear.ctypes.data_as(_P)))
+        return out, bear
+
+    def undistort_keypoints_dev(self, cam, dist, batch, cap, d_kp, d_n_kp, d_undist_out, d_bearings_out=None):
+        """Device-resident form on the arrays OrbExtractor / plp_orb_extract_batch_dev write (device pointers)."""
+        self._check(self._lib.plp_undistort_keypoints_batch_dev(self._h, C.byref(cam), C.byref(dist), C.c_int(batch),
+                                                                C.c_int(cap), d_kp, d_n_kp, d_undist_out, d_bearings_out))
 
     # ------------------------------------------------------------------ match/base.h
     def hamming_matrix(self, a, b):

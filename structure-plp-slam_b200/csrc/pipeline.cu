@@ -7,10 +7,14 @@
 // section 8(e): a live sequence is sequential, so the batch is made of independent tracking problems (offline /
 // multi-sequence mode); each CTA handles one frame.
 //
-// The keypoints of the current frames are taken from the ORB handle's most recent extraction.  Undistortion is
-// the identity here (zero-distortion camera; the host-pointer entry points take undistorted coordinates from
-// the adapter instead).
+// The keypoints of the current frames are taken from the ORB handle's most recent extraction.  A tracker made with a
+// distortion (plp_tracker_create_ex) first undistorts them (camera::*::undistort_keypoints, camera_kernels.cuh) into
+// arrays of its own, so that the grid, the window queries and the pose optimiser's observations read undist_keypts_ as
+// the reference's do (frame.cc:68-86); the octave and angle are those of the ORB keypoints.  Without distortion
+// (plp_tracker_create, or a perspective model with all coefficients 0) undistortion returns every keypoint coordinate
+// bit for bit, so the ORB keypoints are used as they are and no kernel is added.
 #include "common.cuh"
+#include "camera_kernels.cuh"
 #include "match_kernels.cuh"
 #include "pose_kernels.cuh"
 
@@ -222,6 +226,12 @@ __global__ void track_finish_kernel(TrackDev T) {
 
 using namespace plp;
 
+namespace plp {
+plp_status make_undist_job(const plp_camera *cam, const plp_distortion *dist, UndistJob *J);  // camera.cu
+bool distortion_is_identity(const plp_distortion *dist);
+plp_status launch_undistort(plp_ctx *ctx, const UndistJob &J);
+}  // namespace plp
+
 struct plp_tracker {
     plp_ctx *ctx = nullptr;
     int max_batch = 0, cap = 0, max_last = 0, num_levels = 0;
@@ -232,6 +242,10 @@ struct plp_tracker {
     float *d_scale_factors = nullptr;
     uint8_t *d_block = nullptr;  // one allocation carved into the scratch arrays
     TrackDev dev;
+    bool distorted = false;
+    UndistJob undist;                  // camera and coefficients; kp / n_kp / batch set per call
+    plp_keypoint *d_undist = nullptr;  // max_batch x cap (inside d_block)
+    double *d_bearings = nullptr;      // max_batch x cap x 3
 };
 
 extern "C" {
@@ -239,7 +253,17 @@ extern "C" {
 plp_status plp_tracker_create(plp_ctx *ctx, const plp_camera *cam, const plp_grid *grid, const float *scale_factors,
                               const float *inv_level_sigma_sq, int num_levels, int max_batch, int kp_capacity,
                               int max_last_points, plp_tracker **out) {
+    return plp_tracker_create_ex(ctx, cam, grid, scale_factors, inv_level_sigma_sq, num_levels, max_batch, kp_capacity,
+                                 max_last_points, nullptr, out);
+}
+
+plp_status plp_tracker_create_ex(plp_ctx *ctx, const plp_camera *cam, const plp_grid *grid, const float *scale_factors,
+                                 const float *inv_level_sigma_sq, int num_levels, int max_batch, int kp_capacity,
+                                 int max_last_points, const plp_distortion *dist, plp_tracker **out) {
     PLP_REQUIRE(ctx && cam && grid && scale_factors && inv_level_sigma_sq && out, "null pointer");
+    const bool distorted = !distortion_is_identity(dist);
+    UndistJob uj;
+    if (distorted) PLP_TRY(make_undist_job(cam, dist, &uj));
     PLP_REQUIRE(num_levels >= 1 && num_levels <= 16 && max_batch >= 1 && kp_capacity >= 1 && max_last_points >= 1, "sizes");
     PLP_REQUIRE(cam->setup_type == 0, "the batched tracker implements the monocular path");
     *out = nullptr;
@@ -270,6 +294,7 @@ plp_status plp_tracker_create(plp_ctx *ctx, const plp_camera *cam, const plp_gri
     const size_t o_nm = take(B * 4), o_pj = take(2 * B * sizeof(ProjectJob)), o_mj = take(2 * B * sizeof(PointMatchJob));
     const size_t o_poj = take(B * sizeof(PoseJob)), o_obs = take(B * C * sizeof(plp_pt_obs)), o_okp = take(B * C * 4);
     const size_t o_oout = take(B * C);
+    const size_t o_ukp = distorted ? take(B * C * sizeof(plp_keypoint)) : 0, o_ub = distorted ? take(B * C * 24) : 0;
     if (cudaMalloc((void **)&t->d_block, off) != cudaSuccess) {
         set_error("tracker: cudaMalloc(%zu) failed", off);
         delete t;
@@ -303,7 +328,21 @@ plp_status plp_tracker_create(plp_ctx *ctx, const plp_camera *cam, const plp_gri
     T.obs_kp = (int32_t *)(d + o_okp);
     T.obs_outlier = d + o_oout;
     for (int l = 0; l < 16; ++l) T.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
+    if (distorted) {
+        t->distorted = true;
+        t->undist = uj;
+        t->d_undist = (plp_keypoint *)(d + o_ukp);
+        t->d_bearings = (double *)(d + o_ub);
+    }
     *out = t;
+    return PLP_OK;
+}
+
+plp_status plp_tracker_undistorted(const plp_tracker *t, const plp_keypoint **d_undist_kp, const double **d_bearings) {
+    PLP_REQUIRE(t && d_undist_kp && d_bearings, "null pointer");
+    PLP_REQUIRE(t->distorted, "the tracker has no distortion: its undistorted keypoints are the ORB keypoints");
+    *d_undist_kp = t->d_undist;
+    *d_bearings = t->d_bearings;
     return PLP_OK;
 }
 
@@ -346,6 +385,17 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
     T.num_valid = d_num_valid_out;
     T.n_inliers = d_n_inliers_out;
     T.lm_iters = d_lm_iters_out;
+    if (t->distorted) {  // frame.cc:68,79: undist_keypts_ and bearings_ of the current frames
+        UndistJob J = t->undist;
+        J.batch = batch;
+        J.cap = t->cap;
+        J.kp = d_kp;
+        J.n_kp = d_n_kp;
+        J.out = t->d_undist;
+        J.bearings = t->d_bearings;
+        PLP_TRY(launch_undistort(ctx, J));
+        T.kp = t->d_undist;
+    }
     PLP_LAUNCH(ctx, track_prep_kernel, batch, 256, 0, T, margin, 1);
     PLP_CHECK_LAUNCH();
     // first attempt (projection.cc:214-358 with `margin`)

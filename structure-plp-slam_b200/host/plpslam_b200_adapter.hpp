@@ -69,6 +69,23 @@ inline plp_camera camera_of(const PLPSLAM::camera::base *b) {
                       (int32_t)b->setup_type_};
 }
 
+// ---- camera::{perspective,fisheye}::undistort_keypoints + convert_keypoints_to_bearings (data/frame.cc:68, :79) ----------
+// Replaces the two calls of every data::frame constructor.  cam: the camera's fx_, fy_, cx_, cy_ (camera_of() for a
+// perspective camera; for a fisheye camera its own fx_ .. cy_) and img_bounds_; dist: Camera.model and the coefficients
+// as the camera holds them (perspective {0, {k1_, k2_, p1_, p2_, k3_}}, fisheye {1, {k1_, k2_, k3_, k4_, 0}}) -- see
+// INTEGRATION.md for the call site.
+inline void undistort_keypoints(const plp_camera &cam, const plp_distortion &dist, const std::vector<cv::KeyPoint> &keypts,
+                                std::vector<cv::KeyPoint> &undist_keypts,
+                                PLPSLAM::eigen_alloc_vector<PLPSLAM::Vec3_t> &bearings) {
+    const int n = (int)keypts.size();
+    undist_keypts.resize(n);
+    std::vector<double> b(3 * (size_t)n);
+    check(plp_undistort_keypoints(thread_ctx(), &cam, &dist, reinterpret_cast<const plp_keypoint *>(keypts.data()), n,
+                                  reinterpret_cast<plp_keypoint *>(undist_keypts.data()), b.data()));
+    bearings.resize(n);
+    for (int i = 0; i < n; ++i) bearings[i] = PLPSLAM::Vec3_t{b[3 * i], b[3 * i + 1], b[3 * i + 2]};
+}
+
 // ---- feature::orb_extractor::extract (feature/orb_extractor.cc:73-160) -------------------------------------
 struct orb_backend {
     plp_orb *h = nullptr;

@@ -9,7 +9,8 @@ import ctypes as C
 
 import numpy as np
 
-from .capi import KP_DTYPE, Context, OrbExtractor, PlpError, _P, make_camera, make_grid  # noqa: F401
+from .capi import (KP_DTYPE, Context, OrbExtractor, PlpError, _P, make_camera, make_distorted_camera,  # noqa: F401
+                   make_grid)
 
 
 class TrackLast(C.Structure):
@@ -88,15 +89,22 @@ class FrontEnd:
 
     def __init__(self, ctx: Context, rows: int, cols: int, cam, max_batch: int, max_last_points: int = 4096,
                  max_num_keypts=1000, scale_factor=1.2, num_levels=8, ini_fast_thr=20, min_fast_thr=7,
-                 track_ctx: Context | None = None):
+                 track_ctx: Context | None = None, distortion=None):
         """track_ctx: optional second context (stream) for the tracking kernels; extraction stays on `ctx`.  The two
-        streams are chained by plp_ctx_wait_ctx, so extract(k + 1) of ANOTHER FrontEnd can run under track(k)."""
+        streams are chained by plp_ctx_wait_ctx, so extract(k + 1) of ANOTHER FrontEnd can run under track(k).
+        distortion: a capi.Distortion (make_distortion); the tracker then undistorts the keypoints before matching, and
+        cam's bounds and the grid come from the undistorted image corners (capi.make_distorted_camera).  None: the
+        camera has no distortion."""
         self.ctx = ctx
         self.track_ctx = track_ctx if track_ctx is not None else ctx
         self.lib = ctx._lib
         self.rows, self.cols, self.max_batch = rows, cols, max_batch
+        self.distortion = distortion
+        if distortion is not None:
+            cam, self.grid = make_distorted_camera(cam.fx, cam.fy, cam.cx, cam.cy, cols, rows, distortion)
+        else:
+            self.grid = make_grid(cols, rows)
         self.cam = cam
-        self.grid = make_grid(cols, rows)
         self.orb = OrbExtractor(ctx, rows, cols, max_num_keypts, scale_factor, num_levels, ini_fast_thr, min_fast_thr,
                                 max_batch=max_batch)
         self.cap = self.orb.capacity
@@ -104,9 +112,16 @@ class FrontEnd:
         h = C.c_void_p()
         sf = np.ascontiguousarray(self.orb.scale_factors, np.float32)
         isig = np.ascontiguousarray(self.orb.inv_level_sigma_sq, np.float32)
-        ctx._check(self.lib.plp_tracker_create(self.track_ctx.handle, C.byref(cam), C.byref(self.grid), sf.ctypes.data_as(_P),
-                                               isig.ctypes.data_as(_P), C.c_int(num_levels), C.c_int(max_batch),
-                                               C.c_int(self.cap), C.c_int(max_last_points), C.byref(h)))
+        if distortion is None:
+            ctx._check(self.lib.plp_tracker_create(self.track_ctx.handle, C.byref(cam), C.byref(self.grid),
+                                                   sf.ctypes.data_as(_P), isig.ctypes.data_as(_P), C.c_int(num_levels),
+                                                   C.c_int(max_batch), C.c_int(self.cap), C.c_int(max_last_points),
+                                                   C.byref(h)))
+        else:
+            ctx._check(self.lib.plp_tracker_create_ex(self.track_ctx.handle, C.byref(cam), C.byref(self.grid),
+                                                      sf.ctypes.data_as(_P), isig.ctypes.data_as(_P), C.c_int(num_levels),
+                                                      C.c_int(max_batch), C.c_int(self.cap), C.c_int(max_last_points),
+                                                      C.byref(distortion), C.byref(h)))
         self._trk = h
         B = max_batch
         self.d_imgs = DeviceBuffer(ctx, B * rows * cols)
@@ -246,6 +261,22 @@ class FrontEnd:
         kp = self.d_kp.download(KP_DTYPE, (self.max_batch, self.cap))[:batch]
         desc = self.d_desc.download(np.uint8, (self.max_batch, self.cap, 32))[:batch]
         return [(kp[b, :n[b]].copy(), desc[b, :n[b]].copy()) for b in range(batch)]
+
+    def download_undistorted(self, batch: int):
+        """Per frame (undistorted keypoints, bearings) of the last track() -- frame::undist_keypts_ and bearings_.
+        Without a distortion the undistorted keypoints are the ORB keypoints and there is nothing to download."""
+        if self.distortion is None:
+            raise PlpError("FrontEnd without distortion: the ORB keypoints are the undistorted keypoints")
+        kp_p, b_p = C.c_void_p(), C.c_void_p()
+        self.ctx._check(self.lib.plp_tracker_undistorted(self._trk, C.byref(kp_p), C.byref(b_p)))
+        n = self.d_n.download(np.int32, (batch,))
+        if self.track_ctx is not self.ctx:
+            self.ctx.wait(self.track_ctx)
+        kp = np.zeros((batch, self.cap), KP_DTYPE)
+        bear = np.zeros((batch, self.cap, 3), np.float64)
+        self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, kp.ctypes.data_as(_P), kp_p, C.c_size_t(kp.nbytes)))
+        self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, bear.ctypes.data_as(_P), b_p, C.c_size_t(bear.nbytes)))
+        return [(kp[b, :n[b]].copy(), bear[b, :n[b]].copy()) for b in range(batch)]
 
     def download_tracking(self, batch: int):
         self._after_tracking()

@@ -8,9 +8,11 @@ cv2_lsd.npz         cv::LineSegmentDetector(1, 0.5, 0.6, 2, 22.5, 1, 0.6, 1024) 
 orb_mirror.npz      orb_extractor::extract with every third-party stage done by cv2 (tests/test_orb_oracle.py mirror)
 line_extract.npz    LineFeatureTracker::extract_LSD_LBD output of the oracle (whose LSD stage is pinned to cv2 above)
 cv2_lsd_odd.npz     cv2's half-resolution LSD image and LSD segments at sizes with a dimension = 3 (mod 4)
+cv2_undistort.npz   cv2.undistortPointsIter / cv2.fisheye.undistortPoints of seeded points for every camera of
+                    tests/camera_data.py, with the oracle's undistortion and image bounds beside them
 The images are regenerated from their seeds by the tests; only the outputs are stored.
 
-    python tools/gen_golden.py cv2_lsd_odd      # only the named files"""
+    python tools/gen_golden.py cv2_lsd_odd cv2_undistort      # only the named files"""
 import sys
 from pathlib import Path
 
@@ -23,6 +25,7 @@ import oracle_api  # noqa: E402
 import synth  # noqa: E402
 import test_golden  # noqa: E402
 import test_orb_oracle  # noqa: E402
+import camera_data  # noqa: E402
 
 OUT = ROOT / "tests" / "golden"
 
@@ -39,11 +42,23 @@ def lsd_odd():
     np.savez_compressed(OUT / "cv2_lsd_odd.npz", **out)
 
 
+def undistort():
+    orc = oracle_api.Oracle()
+    out = {}
+    for name, (model, cols, rows, K, D) in camera_data.ALL.items():
+        x, y = camera_data.test_points(cols, rows, seed=31, n=1000)
+        out[name + "_cv2"] = np.stack(camera_data.cv2_undistort(model, K, camera_data.coeffs5(D), x, y), 1)
+        out[name + "_oracle"] = np.stack(camera_data.undistort_keypoints(orc, model, K, D, x, y), 1)
+        out[name + "_bounds"] = camera_data.image_bounds(orc, model, K, D, cols, rows)
+    out["cv2_version"] = np.array(cv2.__version__)
+    np.savez_compressed(OUT / "cv2_undistort.npz", **out)
+
+
 def main():
     OUT.mkdir(exist_ok=True)
     if sys.argv[1:]:
         for name in sys.argv[1:]:
-            {"cv2_lsd_odd": lsd_odd}[name]()
+            {"cv2_lsd_odd": lsd_odd, "cv2_undistort": undistort}[name]()
         return
     orc = oracle_api.Oracle()
     tex = synth.make_texture(4321, 240, 320, n_rect=120, n_blob=500)      # the image of __graft_entry__.smoke()
@@ -80,6 +95,7 @@ def main():
     kl, lbd, fn = orc.line_extract(lines)
     np.savez_compressed(OUT / "line_extract.npz", keylines=kl, lbd=lbd, line_functions=fn)
     lsd_odd()
+    undistort()
     for f in sorted(OUT.glob("*.npz")):
         print(f.name, f.stat().st_size, "bytes")
 
