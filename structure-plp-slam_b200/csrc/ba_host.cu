@@ -189,8 +189,7 @@ plp_status plp_ba_create(plp_ctx *ctx, const plp_ba_problem *p, const plp_ba_cfg
     // warp owns a landmark, a point landmark costs one round over its (<= 32) edges, a line landmark one round per edge
     // (numeric Jacobians: 21 evaluations spread over the lanes) plus the same per-landmark tail
     const int n_lm = n_pts + n_lines;
-    int w_point = 4, w_line0 = 8;
-    if (const char *wenv = getenv("PLP_BA_COST_WEIGHTS")) sscanf(wenv, "%d,%d", &w_point, &w_line0);  // tuning aid
+    constexpr int w_point = 4, w_line0 = 8;
     int max_deg = 1;
     std::vector<int> deg_e(n_lm + 1, 0);
     for (int l = 0; l < n_pts; ++l) {

@@ -500,7 +500,6 @@ struct plp_line {
     bool force_global_image = false;
     int grow_variant = 0;  // 0 automatic, 1 one warp per frame, 2 multi-warp rounds (lsd_grow_mw_kernel), 3 out of order (lsd_grow_ooo_kernel)
     int ooo_warps = 0;
-    bool ooo_auto = false;
     bool host_call = false;   // inside the host-pointer entry point (a live frame): automatic mode may take the out-of-order kernel
     bool used_ooo = false;    // the last run did
     int ooo_fallbacks = 0;    // host calls that were re-run with the round protocol after an out-of-order timeout
@@ -547,9 +546,9 @@ static plp_status line_run(plp_line *h, const uint8_t *d_imgs, int batch, size_t
     const bool mw = h->mw_warps >= 2 && batch <= h->mw_max_batch && h->grow_variant != 1 &&
                     (h->grow_variant >= 2 || 2 * batch <= ctx->sm_count);  // half a wave: a second handle (stereo) fits beside it
     // automatic mode takes the out-of-order kernel for a live frame or stereo pair through the host entry point (which re-runs
-    // the frame with the round protocol should the kernel ever give up), elsewhere only with PLP_LSD_OOO=1
+    // the frame with the round protocol should the kernel ever give up)
     const bool ooo = mw && h->ooo_warps >= 2 &&
-                     (h->grow_variant == 3 || (h->grow_variant == 0 && (h->ooo_auto || (h->host_call && batch <= 2))));
+                     (h->grow_variant == 3 || (h->grow_variant == 0 && h->host_call && batch <= 2));
     h->used_ooo = ooo;
     if (ooo) {
         PLP_LAUNCH(ctx, lsd_grow_ooo_kernel, batch, h->ooo_warps * 32, h->ooo_smem, D, h->d_reg_mw);
@@ -665,8 +664,6 @@ plp_status plp_line_create(plp_ctx *ctx, int rows, int cols, int max_batch, plp_
     h->sort_smem = ((size_t)kSortWarps * kBins + kBins) * sizeof(uint32_t);
     const size_t used_bytes = (size_t)((((D.npx + 31) >> 5) + 3) & ~3) * 4;
     D.reg_cap_small = kRegCapSmall;
-    if (const char *ev = getenv("PLP_LSD_REGCAP")) D.reg_cap_small = std::max(64, std::min(kRegCap, atoi(ev)));  // tuning aid
-    h->dev.reg_cap_small = D.reg_cap_small;
     h->grow_smem_noimg = used_bytes + (size_t)D.reg_cap_small * 4;
     h->grow_smem = (size_t)((D.npx + 15) & ~15) + used_bytes + (size_t)kRegCap * 4;
     h->img_smem_ok = h->grow_smem <= 227 * 1024;
@@ -685,8 +682,6 @@ plp_status plp_line_create(plp_ctx *ctx, int rows, int cols, int max_batch, plp_
         const size_t fixed = (size_t)((D.npx + 15) & ~15) + used_bytes + sizeof(MwCtl) + 64, per_warp = used_bytes + (size_t)kMwRegCap * 4;
         const size_t budget = 227 * 1024;
         h->mw_warps = fixed + 2 * per_warp <= budget ? (int)std::min<size_t>(kMwMaxWarps, (budget - fixed) / per_warp) : 0;
-        if (const char *ev = getenv("PLP_LSD_DIRECT")) h->dev.direct_trig = atoi(ev);  // tuning aid
-        if (const char *ev = getenv("PLP_LSD_MW_WARPS")) h->mw_warps = std::max(0, std::min(h->mw_warps, atoi(ev)));  // tuning aid
         h->mw_smem = fixed + (size_t)h->mw_warps * per_warp;
         h->mw_max_batch = h->mw_warps >= 2 ? std::min(max_batch, ctx->sm_count) : 0;
         if (h->mw_warps >= 2) {
@@ -696,8 +691,6 @@ plp_status plp_line_create(plp_ctx *ctx, int rows, int cols, int max_batch, plp_
             const size_t ofixed = (size_t)((D.npx + 15) & ~15) + 3 * used_bytes + (size_t)kOooRegCap * 4 + sizeof(OooEntry) * kOooRing +
                                   sizeof(OooCtl) + 64, oper = used_bytes + (size_t)kOooRegCap * 4;
             h->ooo_warps = ofixed + 2 * oper <= budget ? (int)std::min<size_t>(kMwMaxWarps, (budget - ofixed) / oper) : 0;
-            if (const char *ev = getenv("PLP_LSD_OOO")) h->ooo_auto = atoi(ev) != 0;
-            if (const char *ev = getenv("PLP_LSD_OOO_WARPS")) h->ooo_warps = std::max(0, std::min(h->ooo_warps, atoi(ev)));  // tuning aid
             h->ooo_smem = ofixed + (size_t)h->ooo_warps * oper;
             if (h->ooo_warps >= 2 && so == PLP_OK)
                 so = ensure_smem_optin((const void *)lsd_grow_ooo_kernel, h->ooo_smem, "lsd_grow_ooo_kernel");

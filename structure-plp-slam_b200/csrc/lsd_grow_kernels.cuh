@@ -38,8 +38,7 @@ struct LineDev {
     uint32_t *order;     // npx packed (y<<16|x) seeds, bin desc / raster asc
     int *nseeds;
     uint32_t *reg_xy;    // npx: region entries beyond the shared-memory window
-    int reg_cap_small;   // region window (entries) of lsd_grow_kernel<false>
-    int direct_trig;     // bit 0: lsd_grow_mw_kernel, bit 1: lsd_grow_kernel compute the neighbour's {deg, cos, sin} directly
+    int reg_cap_small;   // region window (entries) of lsd_grow_kernel<false>: kRegCapSmall
     unsigned long long *mw_stat;  // per frame {rounds, seeds run, seeds redone} of lsd_grow_mw_kernel (may be null)
     float4 *segs;        // seg_cap
     int *nseg;
@@ -103,7 +102,6 @@ struct GrowT {  // per-warp state
     uint32_t *reg_ovf;     // global: all entries beyond reg_cap (indexed by absolute position)
     const float4 *tab;     // global: {deg, cos, sin} by (gx, gy)
     int lane, reg_cap;
-    bool direct;           // compute {deg, cos, sin} of a neighbour instead of reading the table
     mutable int bx0, by0, bx1, by1;  // kMw: per-lane bounding box of the pixels this lane accepted (reduced by the caller)
     // out-of-order kernel only (claim == nullptr otherwise): `claim` = union of the private marks of every context in flight;
     // a region that is about to accept a pixel claimed by an EARLIER ticket stops at once (`aborted`) and is decided at the head
@@ -112,9 +110,6 @@ struct GrowT {  // per-warp state
     const int *ctx_ticket;       // ticket each context is working on (INT_MAX: idle)
     int nctx, self, my_ticket, ctx_words;
     mutable bool aborted;
-#ifdef PLP_LSD_PROF
-    long long *pc;         // [0] iterations [1] rounds [2] cycles load phase [3] cycles resolve phase [4] on-demand loads
-#endif
     __device__ __forceinline__ uint32_t get(int e) const { return e < reg_cap ? reg[e] : reg_ovf[e]; }
     __device__ __forceinline__ void put(int e, uint32_t v) const {
         if (e < reg_cap) reg[e] = v;
@@ -197,13 +192,7 @@ __device__ __forceinline__ Nb load_nb(const GrowT<kMw> &G, int e, int ddx, int d
         if (gx * gx + gy * gy > G.kthr) {
             r.nidx = idx;
             r.xy = ((uint32_t)ny << 16) | (uint32_t)nx;
-            if (G.direct) {  // latency mode: ~250 dependent cycles of arithmetic instead of a table entry from L2
-                const float deg = fast_atan2_deg((float)gx, (float)-gy);
-                const double af = (double)(float)((double)deg * kDegToRads);
-                r.t = make_float4(deg, (float)det_cos(af), (float)det_sin(af), 0.f);
-            } else {
-                r.t = G.tab[(gy + kGRange) * kGDim + gx + kGRange];
-            }
+            r.t = G.tab[(gy + kGRange) * kGDim + gx + kGRange];
         }
     }
     return r;
@@ -236,11 +225,6 @@ __device__ int region_grow(const GrowT<kMw> &G, uint32_t seed_xy, float seed_deg
     int loaded = 0;  // groups of `cur` that hold valid data
     while (i < n) {
         const int take = min(4, n - i);
-#ifdef PLP_LSD_PROF
-        const long long tl0 = clock64();
-        G.pc[0]++;
-        if (loaded < take) G.pc[4]++;
-#endif
         if (g >= loaded && g < take) cur = load_nb(G, i + g, ddx, ddy);  // entries that were not known one round ago
         // prefetch the entries already known for the next round
         const int nxt_avail = min(4, n - (i + take));
@@ -250,10 +234,6 @@ __device__ int region_grow(const GrowT<kMw> &G, uint32_t seed_xy, float seed_deg
         nxt.t = make_float4(0.f, 0.f, 0.f, 0.f);
         if (g < nxt_avail) nxt = load_nb(G, i + take + g, ddx, ddy);
         // resolve the current entries
-#ifdef PLP_LSD_PROF
-        const long long tl1 = clock64();
-        G.pc[2] += tl1 - tl0;
-#endif
         bool cand = (g < take) && (cur.nidx >= 0) && !G.is_used(cur.nidx);
         const bool ce = cand && G.claimed_by_earlier(cur.nidx);  // (false unless the out-of-order kernel runs)
         const double a = (double)cur.t.x * kDegToRads;
@@ -263,9 +243,6 @@ __device__ int region_grow(const GrowT<kMw> &G, uint32_t seed_xy, float seed_deg
             const bool al = cand && is_aligned(a, reg_angle, prec);
             const unsigned m = __ballot_sync(kFull, al);
             if (!m) break;
-#ifdef PLP_LSD_PROF
-            G.pc[1]++;
-#endif
             const int l = __ffs(m) - 1;
             if (kMw && __shfl_sync(kFull, ce ? 1 : 0, l)) {  // the next pixel of the sequential order belongs to an earlier region in flight
                 G.aborted = true;
@@ -287,9 +264,6 @@ __device__ int region_grow(const GrowT<kMw> &G, uint32_t seed_xy, float seed_deg
             my_theta = (double)fast_atan2_deg(my_sdy, my_sdx) * kDegToRads;
         }
         __syncwarp();
-#ifdef PLP_LSD_PROF
-        G.pc[3] += clock64() - tl1;
-#endif
         i += take;
         cur = nxt;
         loaded = nxt_avail;
@@ -447,14 +421,6 @@ __device__ bool refine(const GrowT<kMw> &G, int &n, float seed_deg, double reg_a
     return true;
 }
 
-#ifdef PLP_LSD_PROF
-#define PROF_T(var) const long long var = clock64()
-#define PROF_ADD(slot, t0) prof[slot] += clock64() - (t0)
-#else
-#define PROF_T(var)
-#define PROF_ADD(slot, t0)
-#endif
-
 // kImgSmem: the half-resolution image is staged in shared memory (lowest latency, 2 frames per SM at VGA) or read from
 // global memory through L1 / L2 (34 KB of shared memory per frame -> 6 frames per SM: more frames in flight for big
 // batches; the images of a batch, 77 KB each, stay L2 resident)
@@ -462,13 +428,6 @@ template <bool kImgSmem>
 __global__ void __launch_bounds__(32) lsd_grow_kernel(LineDev D) {
     PLP_DYNAMIC_SMEM(s_grow_raw);
     uint4 *s_grow = reinterpret_cast<uint4 *>(s_grow_raw);
-#ifdef PLP_LSD_PROF
-    long long prof[6] = {0, 0, 0, 0, 0, 0};
-    long long cnt_regions = 0, cnt_px = 0, cnt_refine = 0;
-    __shared__ long long s_pc[8];
-    for (int q = 0; q < 8; ++q) s_pc[q] = 0;
-    const long long t_start = clock64();
-#endif
     uint8_t *s_img = reinterpret_cast<uint8_t *>(s_grow);
     const int img_bytes = kImgSmem ? ((D.npx + 15) & ~15) : 0;
     uint32_t *s_used = reinterpret_cast<uint32_t *>(s_img + img_bytes);
@@ -501,12 +460,8 @@ __global__ void __launch_bounds__(32) lsd_grow_kernel(LineDev D) {
     G.reg = s_reg;
     G.reg_ovf = D.reg_xy + (size_t)b * D.npx;
     G.tab = D.cstab;
-    G.direct = (D.direct_trig & 2) != 0;
     G.claim = nullptr;
     G.aborted = false;
-#ifdef PLP_LSD_PROF
-    G.pc = s_pc;
-#endif
     G.lane = lane;
     const uint32_t *order = D.order + (size_t)b * D.npx;
     float4 *segs = D.segs + (size_t)b * D.seg_cap;
@@ -526,24 +481,11 @@ __global__ void __launch_bounds__(32) lsd_grow_kernel(LineDev D) {
             grad_at(G.img, sw, sidx, gx, gy);
             const float seed_deg = fast_atan2_deg((float)gx, (float)-gy);
             double reg_angle;
-            PROF_T(t0);
             int n = region_grow(G, seed_xy, seed_deg, D.prec, reg_angle);
-            PROF_ADD(0, t0);
-#ifdef PLP_LSD_PROF
-            cnt_regions++;
-            cnt_px += n;
-#endif
             if (n >= D.min_reg_size) {
                 Rect R;
-                PROF_T(t1);
                 region2rect(G, n, reg_angle, D.prec, R);
-                PROF_ADD(1, t1);
-                PROF_T(t2);
                 const bool okr = refine(G, n, seed_deg, reg_angle, D.prec, R);
-                PROF_ADD(2, t2);
-#ifdef PLP_LSD_PROF
-                cnt_refine++;
-#endif
                 if (okr) {
                     if (nseg < D.seg_cap) {
                         if (lane == 0) {
@@ -562,11 +504,6 @@ __global__ void __launch_bounds__(32) lsd_grow_kernel(LineDev D) {
         }
     }
     if (lane == 0) D.nseg[b] = min(nseg, D.seg_cap);
-#ifdef PLP_LSD_PROF
-    if (lane == 0 && b == 0)
-        printf("[lsd prof] total %lld grow %lld rect %lld refine %lld | seeds %d regions %lld px %lld big %lld segs %d | iters %lld rounds %lld load-cyc %lld resolve-cyc %lld ondemand %lld\n",
-               clock64() - t_start, prof[0], prof[1], prof[2], nseeds, cnt_regions, cnt_px, cnt_refine, nseg, s_pc[0], s_pc[1], s_pc[2], s_pc[3], s_pc[4]);
-#endif
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -632,7 +569,6 @@ __global__ void __launch_bounds__(kMwMaxWarps * 32) lsd_grow_mw_kernel(LineDev D
     G.reg = s_reg + (size_t)warp * kMwRegCap;
     G.reg_ovf = reg_ovf_mw + ((size_t)b * kMwMaxWarps + warp) * D.npx;
     G.tab = D.cstab;
-    G.direct = (D.direct_trig & 1) != 0;
     G.claim = nullptr;
     G.aborted = false;
     G.lane = lane;
@@ -1052,7 +988,6 @@ __global__ void __launch_bounds__(kMwMaxWarps * 32) lsd_grow_ooo_kernel(LineDev 
     G.reg_cap = kOooRegCap;
     G.used = s_used;
     G.tab = D.cstab;
-    G.direct = false;
     G.lane = lane;
     G.claim = s_claim;
     G.priv_base = s_priv;

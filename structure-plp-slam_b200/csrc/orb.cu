@@ -114,15 +114,6 @@ struct BlurMaps {
 
 __device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// the descriptor of level l: a kernel parameter (__grid_constant__) or, with PLP_TMA_MAPS=global, an array in device
-// memory (acquired through the tensormap proxy, since the level-0 entry is rewritten when the caller's buffer changes)
-template <bool kMapsInGlobal>
-__device__ __forceinline__ const CUtensorMap *level_map(const BlurMaps &M, const CUtensorMap *gmaps, int l) {
-    const CUtensorMap *tm = kMapsInGlobal ? gmaps + l : &M.m[l];
-    if (kMapsInGlobal) asm volatile("fence.proxy.tensormap::generic.acquire.gpu [%0], 128;" ::"l"(tm) : "memory");
-    return tm;
-}
-
 __device__ __forceinline__ void mbar_init(uint32_t bar) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(bar)); }
 
 // bounded wait for phase `parity` of an mbarrier; false if it did not complete (the copy never arrived)
@@ -499,8 +490,8 @@ __device__ __forceinline__ void fast_cell_emit(const OrbDev &P, int b, int ci, F
     if (tid == 0) P.cell_cnt[(size_t)b * P.num_cells + ci] = min(S.wsum[0] + S.wsum[1] + S.wsum[2] + S.wsum[3], kCellCap);
 }
 
-// one cell per CTA, the tile by plain loads: the path for caller buffers TMA cannot describe (and the A/B reference of
-// fast_cells_tma_kernel, PLP_BLUR_NO_TMA=1).  Level pitches are 64-byte multiples, so with a 16-byte aligned level the
+// one cell per CTA, the tile by plain loads: the path for caller buffers TMA cannot describe (a base or pitch that is
+// not a multiple of 16 bytes).  Level pitches are 64-byte multiples, so with a 16-byte aligned level the
 // tile rows are fetched as aligned 16-byte chunks from min_x - kTileX: they read [min_x - 3, min_x + w + 13) at most,
 // left of which lie >= 16 border pixels, and max_x + 15 <= cols - 4, so no read leaves the image row.
 __global__ void __launch_bounds__(256, 4) fast_cells_kernel_v2(OrbDev P) {
@@ -540,9 +531,7 @@ __global__ void __launch_bounds__(256, 4) fast_cells_kernel_v2(OrbDev P) {
 // The grid is not persistent: short runs keep CTAs retiring, so that kernels of a concurrent higher-priority stream
 // (the tracking of the other sub-batch in the front end) still get SMs.
 constexpr int kFastRun = 4;
-template <bool kMapsInGlobal>
-__global__ void __launch_bounds__(256, 4) fast_cells_tma_kernel(const __grid_constant__ BlurMaps M, const CUtensorMap *gmaps,
-                                                                 OrbDev P, int run) {
+__global__ void __launch_bounds__(256, 4) fast_cells_tma_kernel(const __grid_constant__ BlurMaps M, OrbDev P, int run) {
     __shared__ __align__(128) uint8_t s_tile[2][kFastStage];
     __shared__ FastSmem S;
     __shared__ __align__(8) unsigned long long s_bar[2];
@@ -558,7 +547,7 @@ __global__ void __launch_bounds__(256, 4) fast_cells_tma_kernel(const __grid_con
     auto issue = [&](int i) {  // thread 0: the tile of cell first + i into stage i & 1
         const CellDesc c = P.cells[first + i];
         const uint32_t bar = smem_u32(&s_bar[i & 1]), dst = smem_u32(s_tile[i & 1]);
-        const CUtensorMap *tm = level_map<kMapsInGlobal>(M, gmaps, c.level);
+        const CUtensorMap *tm = &M.m[c.level];
         mbar_expect_tx(bar, 2 * kBoxH * kBoxW);
         tma_box_load(dst, tm, c.min_x - kTileX, c.min_y, b, bar);
         tma_box_load(dst + kFastBox2Row * kTilePitch, tm, c.min_x - kTileX, c.min_y + kFastBox2Row, b, bar);
@@ -1324,9 +1313,7 @@ __device__ void blur_reflect_box(uint8_t *box, int bx0, int by0, int W, int H) {
 // tiles per CTA: 4, 8 and 16 give the same blur time (0.34 ms per 256-frame sub-batch on one H100 80GB HBM3 at 400 W);
 // 4 gave the best step time of the front end, whose tracking stream needs SMs while the blur runs
 constexpr int kBlurRun = 4;
-template <bool kMapsInGlobal>
-__global__ void __launch_bounds__(kBlurThreads) blur_tiles_tma_kernel(const __grid_constant__ BlurMaps M, const CUtensorMap *gmaps,
-                                                                      OrbDev P, int run) {
+__global__ void __launch_bounds__(kBlurThreads) blur_tiles_tma_kernel(const __grid_constant__ BlurMaps M, OrbDev P, int run) {
     __shared__ __align__(128) uint8_t s_src[2][kBoxStage];
     __shared__ __align__(16) uint32_t s_h2[(kBoxH / 2) * kBtW];
     __shared__ __align__(8) unsigned long long s_bar[2];
@@ -1342,7 +1329,7 @@ __global__ void __launch_bounds__(kBlurThreads) blur_tiles_tma_kernel(const __gr
         const BlurTile t = P.blur_tiles[first + i];
         const uint32_t bar = smem_u32(&s_bar[i & 1]);
         mbar_expect_tx(bar, kBoxH * kBoxW);
-        tma_box_load(smem_u32(s_src[i & 1]), level_map<kMapsInGlobal>(M, gmaps, t.level), t.x0 - kBoxX, t.y0 - 3, b, bar);
+        tma_box_load(smem_u32(s_src[i & 1]), &M.m[t.level], t.x0 - kBoxX, t.y0 - 3, b, bar);
     };
     if (tid == 0) issue(0);
     for (int i = 0; i < n; ++i) {
@@ -1618,10 +1605,6 @@ struct plp_orb {
     // level 0 is the caller's buffer (re-encoded when its address / pitch / batch changes)
     BlurMaps maps;
     bool maps_ok = false;       // levels >= 1 encoded
-    bool no_tma = false;        // PLP_BLUR_NO_TMA=1
-    bool maps_global = false;   // PLP_TMA_MAPS=global: descriptors read from device memory instead of kernel parameters
-    CUtensorMap *d_maps = nullptr;
-    bool d_maps_dirty = true;
     const uint8_t *map0_img = nullptr;
     size_t map0_step = 0;
     int map0_batch = 0;
@@ -1707,7 +1690,7 @@ void plp_orb_destroy(plp_orb *o) {
         if (o->d_ytab[l]) cudaFree(o->d_ytab[l]);
     }
     void *ptrs[] = {o->d_blur, o->d_blur_tiles, o->d_cells, o->d_pyr, o->d_img, o->d_mask, o->d_cell_buf, o->d_cell_cnt, o->d_lvl_kp,
-                    o->d_lvl_cnt, o->d_qt_scratch, o->d_status, o->d_kp, o->d_desc, o->d_n, o->d_maps};
+                    o->d_lvl_cnt, o->d_qt_scratch, o->d_status, o->d_kp, o->d_desc, o->d_n};
     for (void *p : ptrs)
         if (p) cudaFree(p);
     delete o;
@@ -1726,12 +1709,6 @@ plp_status plp_orb_create(plp_ctx *ctx, const plp_orb_params *params, int rows, 
                 "FAST thresholds: 1 <= min <= ini < 255");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     plp_orb *o = new plp_orb();
-    {
-        const char *nt = getenv("PLP_BLUR_NO_TMA");
-        o->no_tma = nt && nt[0] == '1';
-        const char *mg = getenv("PLP_TMA_MAPS");
-        o->maps_global = mg && mg[0] == 'g';
-    }
     o->ctx = ctx;
     o->params = *params;
     o->rows = rows;
@@ -1910,7 +1887,6 @@ plp_status plp_orb_create(plp_ctx *ctx, const plp_orb_params *params, int rows, 
     D.qt_scratch_per_job = (size_t)65536 * (4 + 2 * 5 + 1) + 256;
     ORB_ALLOC(o->d_qt_scratch, B * L * D.qt_scratch_per_job);
     ORB_ALLOC(o->d_status, B * sizeof(int));
-    ORB_ALLOC(o->d_maps, sizeof(BlurMaps));
     ORB_ALLOC(o->d_kp, B * (size_t)D.out_cap * sizeof(plp_keypoint));
     ORB_ALLOC(o->d_desc, B * (size_t)D.out_cap * 32);
     ORB_ALLOC(o->d_n, B * sizeof(int32_t));
@@ -1931,7 +1907,7 @@ plp_status plp_orb_create(plp_ctx *ctx, const plp_orb_params *params, int rows, 
     for (unsigned l = 1; l < L && o->maps_ok; ++l)
         o->maps_ok = encode_level_map(&o->maps.m[l], o->d_pyr + D.lv[l].offset, D.lv[l].w, D.lv[l].h, max_batch, D.lv[l].pitch,
                                       D.pyr_frame_bytes);
-    o->qt_small = qt_max_slots <= kNodeCapSmall && !getenv("PLP_QT_LARGE");
+    o->qt_small = qt_max_slots <= kNodeCapSmall;
     plp_status so;
     if (o->qt_small) {
         o->qt_smem = ((sizeof(QtSharedT<kNodeCapSmall>) + 15) & ~(size_t)15) + (size_t)kCandCapSmall * (4 + 2 * 5 + 1) + 64;
@@ -1983,34 +1959,25 @@ static plp_status orb_run(plp_orb *o, const uint8_t *d_imgs, int batch, size_t s
         PLP_LAUNCH(ctx, pyr_resize_kernel, grid, 256, 0, D, l, o->d_xtab[l], o->d_ytab[l]);
     }
     // TMA descriptors for the FAST tiles and the blur boxes: level 0 is the caller's buffer
-    bool tma = o->maps_ok && !o->no_tma;
+    bool tma = o->maps_ok;
     if (tma && (o->map0_img != d_imgs || o->map0_step != step || o->map0_batch != batch)) {
         tma = encode_level_map(&o->maps.m[0], d_imgs, D.lv[0].w, D.lv[0].h, batch, step, D.img0_frame_stride);
         o->map0_img = tma ? d_imgs : nullptr;
-        o->d_maps_dirty = true;
         o->map0_step = step;
         o->map0_batch = batch;
     }
-    if (tma && o->maps_global && o->d_maps_dirty) {
-        PLP_CUDA_TRY(cudaMemcpyAsync(o->d_maps, &o->maps, sizeof(BlurMaps), cudaMemcpyHostToDevice, ctx->stream));
-        o->d_maps_dirty = false;
-    }
-    // without TMA (caller buffer not 16-byte aligned / pitched, or PLP_BLUR_NO_TMA=1 for A/B runs): plain loads
+    // without TMA (caller buffer not 16-byte aligned / pitched): plain loads
     if (D.num_cells > 0) {
         dim3 grid(D.num_cells, batch), grid_run(div_up(D.num_cells, kFastRun), batch);
-        if (tma && o->maps_global)
-            PLP_LAUNCH(ctx, fast_cells_tma_kernel<true>, grid_run, 256, 0, o->maps, o->d_maps, D, kFastRun);
-        else if (tma)
-            PLP_LAUNCH(ctx, fast_cells_tma_kernel<false>, grid_run, 256, 0, o->maps, (const CUtensorMap *)nullptr, D, kFastRun);
+        if (tma)
+            PLP_LAUNCH(ctx, fast_cells_tma_kernel, grid_run, 256, 0, o->maps, D, kFastRun);
         else
             PLP_LAUNCH(ctx, fast_cells_kernel_v2, grid, 256, 0, D);
     }
     if (D.num_blur_tiles > 0) {
         dim3 grid(D.num_blur_tiles, batch), grid_run(div_up(D.num_blur_tiles, kBlurRun), batch);
-        if (tma && o->maps_global)
-            PLP_LAUNCH(ctx, blur_tiles_tma_kernel<true>, grid_run, kBlurThreads, 0, o->maps, o->d_maps, D, kBlurRun);
-        else if (tma)
-            PLP_LAUNCH(ctx, blur_tiles_tma_kernel<false>, grid_run, kBlurThreads, 0, o->maps, (const CUtensorMap *)nullptr, D, kBlurRun);
+        if (tma)
+            PLP_LAUNCH(ctx, blur_tiles_tma_kernel, grid_run, kBlurThreads, 0, o->maps, D, kBlurRun);
         else
             PLP_LAUNCH(ctx, blur_tiles_kernel, grid, kBlurThreads, 0, D);
     }

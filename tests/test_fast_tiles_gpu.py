@@ -1,10 +1,10 @@
 """The FAST cell tiles arrive two ways: by TMA bulk tensor copies in runs of cells per CTA (fast_cells_tma_kernel, the
-default) and by plain loads, one cell per CTA (fast_cells_kernel_v2: caller buffers TMA cannot describe, and every buffer
-under PLP_BLUR_NO_TMA=1).  Both must give the oracle's candidates, keypoints and descriptors bit for bit, at the
-benchmark's batch and at the edges of the run logic: a run crossing a level boundary, a partial last run, masked cells,
-the fallback threshold, and a frame whose candidates overflow the quadtree's clip."""
-import os
-
+default) and by plain loads, one cell per CTA (fast_cells_kernel_v2, for caller buffers TMA cannot describe: a base or
+pitch that is not a multiple of 16 bytes).  The plain-load arms reach that kernel the way a caller does: through the
+device entry point from a buffer one byte past a 16-byte boundary, or through the host entry points (which stage the
+frames at pitch `cols`) at a width that is not a multiple of 16.  Both paths must give the oracle's candidates, keypoints
+and descriptors bit for bit, at the benchmark's batch and at the edges of the run logic: a run crossing a level boundary,
+a partial last run, masked cells, the fallback threshold, and a frame whose candidates overflow the quadtree's clip."""
 import numpy as np
 import pytest
 
@@ -15,6 +15,7 @@ from test_batch_dev_gpu import _OrbOut, _bench, _kernels_run, _pitched
 pytestmark = pytest.mark.gpu
 RUN = 4  # cells per CTA of fast_cells_tma_kernel (kFastRun in csrc/orb.cu)
 MAX_ROWS, MAX_COLS = 1061, 2085
+PLAIN_COLS = 632  # not a multiple of 16: the host entry points stage such frames at a pitch TMA cannot describe
 
 
 @pytest.fixture
@@ -25,17 +26,16 @@ def own():
         (x.free if hasattr(x, "free") else x.close)()
 
 
-def _plain_loads(plp, ctx, *args, **kw):
-    """An extractor created under PLP_BLUR_NO_TMA=1 (read at create): every tile by plain loads."""
-    old = os.environ.get("PLP_BLUR_NO_TMA")
-    os.environ["PLP_BLUR_NO_TMA"] = "1"
-    try:
-        return plp.OrbExtractor(ctx, *args, **kw)
-    finally:
-        if old is None:
-            del os.environ["PLP_BLUR_NO_TMA"]
-        else:
-            os.environ["PLP_BLUR_NO_TMA"] = old
+def _run_plain(ctx, plp, run):
+    """Run `run`, which must take the plain-load FAST and blur kernels and no TMA kernel."""
+    names = _kernels_run(ctx, plp.lib(), run)
+    assert {"fast_cells_kernel_v2", "blur_tiles_kernel"} <= names and not any("_tma_" in k for k in names), names
+
+
+def _run_tma(ctx, plp, run):
+    """Run `run`, which must take the TMA FAST kernel."""
+    names = _kernels_run(ctx, plp.lib(), run)
+    assert any(k.startswith("fast_cells_tma_kernel") for k in names), names
 
 
 def _cells_per_level(orc, p, rows, cols):
@@ -80,22 +80,26 @@ def _check_oracle(orc, p, img, ext, b, got, mask=None):
     assert np.array_equal(desc, r["desc"]), f"frame {b}: descriptors"
 
 
-def test_bench_batch_tma_equals_plain_loads_and_oracle(ctx, orc, plp, own):
+def test_bench_batch_tma_equals_unaligned_plain_loads_and_oracle(ctx, orc, plp, own):
     """One 256-frame sub-batch of the benchmark's inputs.  At 640 x 480 the frame's 216 cells are 54 full runs, and
-    level 0's 70 cells end in the middle of a run, so runs cross levels."""
+    level 0's 70 cells end in the middle of a run, so runs cross levels.  The plain-load arm reads the same frames from a
+    caller buffer one byte past a 16-byte boundary; its status array must be all zero, as the host call's is (that call
+    fails on a non-zero status)."""
     _, frames, _ = _bench().build_inputs(256, 1234)
     B, rows, cols = frames.shape
     p = oracle_api.orb_params()
     cells = _cells_per_level(orc, p, rows, cols)
     assert sum(cells) == 216 and cells[0] % RUN != 0
-    lib = plp.lib()
     tma = own(plp.OrbExtractor(ctx, rows, cols, max_batch=B))
-    plain = own(_plain_loads(plp, ctx, rows, cols, max_batch=B))
-    got_t, got_p = {}, {}
-    names = _kernels_run(ctx, lib, lambda: got_t.update(enumerate(tma.extract_batch(frames))))
-    assert any(k.startswith("fast_cells_tma_kernel") for k in names), names
-    names = _kernels_run(ctx, lib, lambda: got_p.update(enumerate(plain.extract_batch(frames))))
-    assert "fast_cells_kernel_v2" in names and not any(k.startswith("fast_cells_tma") for k in names), names
+    plain = own(plp.OrbExtractor(ctx, rows, cols, max_batch=B))
+    got_t = {}
+    _run_tma(ctx, plp, lambda: got_t.update(enumerate(tma.extract_batch(frames))))
+    out = own(_OrbOut(plp, ctx, B, plain.capacity))
+    d_img, ptr = _pitched(ctx, frames, cols, offset=1)
+    own(d_img)
+    _run_plain(ctx, plp, lambda: out.run(plain, ptr, B, cols))
+    _, got_p, st = out.get(plp, B)
+    assert not st.any(), st
     for b in range(B):
         _same_candidates(_candidates(tma, b, 8), _candidates(plain, b, 8), f"frame {b}")
         assert np.array_equal(got_t[b][0], got_p[b][0]), f"frame {b}: keypoints"
@@ -108,18 +112,19 @@ def test_bench_batch_tma_equals_plain_loads_and_oracle(ctx, orc, plp, own):
 def test_other_sizes_and_partial_last_run(ctx, orc, plp, own, rows, cols):
     """752 x 480 (EuRoC): 256 cells per frame, runs crossing the boundaries of levels 4 to 6.  512 x 512 (TUM-VI): 174
     cells, so the last CTA of a frame has a partial run.  A caller buffer and status array: status 0 (3 would be a tile
-    copy that never arrived)."""
+    copy that never arrived).  The plain-load arm reads a buffer one byte past a 16-byte boundary."""
     p = oracle_api.orb_params()
     cells = _cells_per_level(orc, p, rows, cols)
     assert (sum(cells) % RUN != 0) == (cols == 512)
     imgs = np.stack([synth.make_texture(60 + i, rows, cols) for i in range(3)] +
                     [synth.make_plp_texture(63, rows, cols), synth.make_line_image(64, rows, cols)])
     B = len(imgs)
-    for ext in (own(plp.OrbExtractor(ctx, rows, cols, max_batch=B)), own(_plain_loads(plp, ctx, rows, cols, max_batch=B))):
+    for offset, check in ((0, _run_tma), (1, _run_plain)):
+        ext = own(plp.OrbExtractor(ctx, rows, cols, max_batch=B))
         out = own(_OrbOut(plp, ctx, B, ext.capacity))
-        d_img, ptr = _pitched(ctx, imgs, cols)
+        d_img, ptr = _pitched(ctx, imgs, cols, offset=offset)
         own(d_img)
-        out.run(ext, ptr, B, cols)
+        check(ctx, plp, lambda: out.run(ext, ptr, B, cols))
         n, got, st = out.get(plp, B)
         assert not st.any(), st
         for b in range(B):
@@ -128,7 +133,8 @@ def test_other_sizes_and_partial_last_run(ctx, orc, plp, own, rows, cols):
 
 def test_mask_and_fallback_threshold(ctx, orc, plp, own):
     """A mask (cells whose corners are masked are skipped, keypoints under the mask dropped) and a low-contrast frame
-    where about half of the cells find no corner at the initial threshold and fall back to the minimum one."""
+    where about half of the cells find no corner at the initial threshold and fall back to the minimum one.  The
+    plain-load arm takes the same frames and mask cropped to a width TMA cannot describe."""
     rows, cols = 480, 640
     p = oracle_api.orb_params()
     tex = synth.make_texture(71)
@@ -136,9 +142,12 @@ def test_mask_and_fallback_threshold(ctx, orc, plp, own):
     mask = np.ones((rows, cols), np.uint8)
     mask[100:260, 200:420] = 0
     mask[400:, :90] = 0
-    for ext in (own(plp.OrbExtractor(ctx, rows, cols)), own(_plain_loads(plp, ctx, rows, cols))):
+    for w, check in ((cols, _run_tma), (PLAIN_COLS, _run_plain)):
+        ext = own(plp.OrbExtractor(ctx, rows, w))
         for img, mk in ((tex, mask), (weak, None), (weak, mask)):
-            got = ext.extract(img, mk)
+            img, mk = np.ascontiguousarray(img[:, :w]), None if mk is None else np.ascontiguousarray(mk[:, :w])
+            got = []
+            check(ctx, plp, lambda: got.extend(ext.extract(img, mk)))
             _check_oracle(orc, p, img, ext, 0, got, mask=mk)
     r = orc.orb_extract(p, weak, debug=True)
     assert 0 < (r["cands"]["response"] < 20).sum() < len(r["cands"])
@@ -172,7 +181,8 @@ def _skipped_cells(orc, p, rows, cols, mask):
 
 def test_masked_cells_inside_runs(ctx, orc, plp, own):
     """Cells skipped by the mask in the middle of a run: the TMA kernel writes the previous cell's output while it
-    starts on the skipped one, whose (empty) counts must not overwrite what that output still reads."""
+    starts on the skipped one, whose (empty) counts must not overwrite what that output still reads.  The plain-load arm
+    takes the same frames and mask cropped to a width TMA cannot describe."""
     rows, cols = 480, 640
     p = oracle_api.orb_params()
     rng = np.random.default_rng(97)
@@ -184,19 +194,20 @@ def test_masked_cells_inside_runs(ctx, orc, plp, own):
     inside = [c for c in range(1, len(skip)) if c % RUN != 0 and skip[c] and not skip[c - 1]]
     assert len(inside) >= 5, inside
     frames = [synth.make_texture(100 + i) for i in range(4)] + [synth.make_plp_texture(104)]
-    tma, plain = own(plp.OrbExtractor(ctx, rows, cols)), own(_plain_loads(plp, ctx, rows, cols))
-    for k, img in enumerate(frames):
-        got_t = tma.extract(img, mask)
-        got_p = plain.extract(img, mask)
-        _same_candidates(_candidates(tma, 0, 8), _candidates(plain, 0, 8), f"frame {k}")
+    tma, plain = own(plp.OrbExtractor(ctx, rows, cols)), own(plp.OrbExtractor(ctx, rows, PLAIN_COLS))
+    mask_p = np.ascontiguousarray(mask[:, :PLAIN_COLS])
+    for img in frames:
+        got_t, got_p = [], []
+        _run_tma(ctx, plp, lambda: got_t.extend(tma.extract(img, mask)))
         _check_oracle(orc, p, img, tma, 0, got_t, mask=mask)
-        assert np.array_equal(got_t[0], got_p[0]) and np.array_equal(got_t[1], got_p[1]), f"frame {k}"
+        img_p = np.ascontiguousarray(img[:, :PLAIN_COLS])
+        _run_plain(ctx, plp, lambda: got_p.extend(plain.extract(img_p, mask_p)))
+        _check_oracle(orc, p, img_p, plain, 0, got_p, mask=mask_p)
 
 
 def test_unaligned_caller_buffer_takes_plain_loads(ctx, orc, plp, own):
     """A caller buffer one byte past an aligned address cannot be described by TMA: the plain-load kernel serves every
     level, with the same candidates as the TMA path on an aligned copy of the frames."""
-    lib = plp.lib()
     imgs = np.stack([synth.make_texture(80 + i) for i in range(3)] + [synth.make_plp_texture(84)])
     B, rows, cols = imgs.shape
     ext_a = own(plp.OrbExtractor(ctx, rows, cols, max_batch=B))
@@ -206,10 +217,8 @@ def test_unaligned_caller_buffer_takes_plain_loads(ctx, orc, plp, own):
     d_u, pu = _pitched(ctx, imgs, cols, offset=1, seed=3)
     own(d_a)
     own(d_u)
-    names = _kernels_run(ctx, lib, lambda: out_a.run(ext_a, pa, B, cols))
-    assert any(k.startswith("fast_cells_tma_kernel") for k in names), names
-    names = _kernels_run(ctx, lib, lambda: out_u.run(ext_u, pu, B, cols))
-    assert "fast_cells_kernel_v2" in names and not any(k.startswith("fast_cells_tma") for k in names), names
+    _run_tma(ctx, plp, lambda: out_a.run(ext_a, pa, B, cols))
+    _run_plain(ctx, plp, lambda: out_u.run(ext_u, pu, B, cols))
     _, got_a, st_a = out_a.get(plp, B)
     _, got_u, st_u = out_u.get(plp, B)
     assert not st_a.any() and not st_u.any(), (st_a, st_u)
@@ -220,17 +229,18 @@ def test_unaligned_caller_buffer_takes_plain_loads(ctx, orc, plp, own):
 
 
 def test_noise_clip_status(ctx, orc, plp, own):
-    """2085 x 1061 noise overflows the 65 535-candidate clip of level 0: status 1 on that frame only, on both paths.
-    640 x 480 noise stays below it."""
+    """2085 x 1061 noise overflows the 65 535-candidate clip of level 0: status 1 on that frame only, on both paths (the
+    plain-load arm reads a buffer one byte past a 16-byte boundary).  640 x 480 noise stays below it, and so does its
+    632-pixel-wide crop, which takes the plain loads."""
     noise = np.random.default_rng(91).integers(0, 256, (MAX_ROWS, MAX_COLS), dtype=np.uint8)
     imgs = np.stack([synth.make_texture(92, MAX_ROWS, MAX_COLS), noise, synth.make_texture(93, MAX_ROWS, MAX_COLS)])
     cands = []
-    for ext in (own(plp.OrbExtractor(ctx, MAX_ROWS, MAX_COLS, 2000, max_batch=3)),
-                own(_plain_loads(plp, ctx, MAX_ROWS, MAX_COLS, 2000, max_batch=3))):
+    for offset, check in ((0, _run_tma), (1, _run_plain)):
+        ext = own(plp.OrbExtractor(ctx, MAX_ROWS, MAX_COLS, 2000, max_batch=3))
         out = own(_OrbOut(plp, ctx, 3, ext.capacity))
-        d_img, ptr = _pitched(ctx, imgs, MAX_COLS + 11, seed=9)
+        d_img, ptr = _pitched(ctx, imgs, MAX_COLS + 11, offset=offset, seed=9)
         own(d_img)
-        out.run(ext, ptr, 3, MAX_COLS + 11)
+        check(ctx, plp, lambda: out.run(ext, ptr, 3, MAX_COLS + 11))
         _, _, st = out.get(plp, 3)
         assert list(st) == [0, 1, 0], st
         cands.append([_candidates(ext, b, 8) for b in range(3)])
@@ -238,6 +248,8 @@ def test_noise_clip_status(ctx, orc, plp, own):
         _same_candidates(cands[0][b], cands[1][b], f"2085 x 1061 frame {b}")
     small = np.random.default_rng(94).integers(0, 256, (480, 640), dtype=np.uint8)
     p = oracle_api.orb_params()
-    for ext in (own(plp.OrbExtractor(ctx, 480, 640)), own(_plain_loads(plp, ctx, 480, 640))):
-        got = ext.extract(small)
-        _check_oracle(orc, p, small, ext, 0, got)
+    for w, check in ((640, _run_tma), (PLAIN_COLS, _run_plain)):
+        ext = own(plp.OrbExtractor(ctx, 480, w))
+        img, got = np.ascontiguousarray(small[:, :w]), []
+        check(ctx, plp, lambda: got.extend(ext.extract(img)))
+        _check_oracle(orc, p, img, ext, 0, got)

@@ -14,26 +14,19 @@ from plpslam_b200.ba import LocalBA  # noqa: E402
 
 ctx = plp.Context(0)
 lib = plp.lib()
-import os  # noqa: E402
-
-for ctas, weights in ((0, None), (0, "4,8"), (0, "4,16"), (0, "2,8"), (0, "4,32"), (0, "8,16")):
-    if weights:
-        os.environ["PLP_BA_COST_WEIGHTS"] = weights  # cost model of the CTA landmark ranges (ba_host.cu)
-    else:
-        os.environ.pop("PLP_BA_COST_WEIGHTS", None)
-    prob = ba_data.make_ba_problem(42)
-    st = prob.struct()
-    ba = LocalBA(ctx, st, (len(prob.kf_fixed), len(prob.pt_pos_w), len(prob.line_plucker), len(prob.pt_edge_kf),
-                           len(prob.line_edge_kf)), num_ctas=ctas)
-    ba.bench_tries(15)
-    ctx._check(lib.plp_ctx_kernel_timing(ctx.handle, 1))
-    ba.bench_tries(30)
-    buf = C.create_string_buffer(1 << 16)
-    ctx._check(lib.plp_ctx_kernel_timing_report(ctx.handle, buf, C.c_size_t(len(buf))))
-    ctx._check(lib.plp_ctx_kernel_timing(ctx.handle, 0))
-    kt = json.loads(buf.value.decode())
-    tot = sum(v["total_ms"] for v in kt.values())
-    print(f"num_ctas={ctas} weights={weights}: total {tot:.3f} ms for 31 tries -> {tot / 31 * 1e3:.1f} us/try")
-    for k, v in sorted(kt.items(), key=lambda kv: -kv[1]["total_ms"]):
-        print(f"   {k:28s} n={v['count']:4d} mean_us={1e3 * v['total_ms'] / v['count']:8.1f} share={v['total_ms'] / tot:.3f}")
-    ba.close()
+prob = ba_data.make_ba_problem(42)
+st = prob.struct()
+ba = LocalBA(ctx, st, (len(prob.kf_fixed), len(prob.pt_pos_w), len(prob.line_plucker), len(prob.pt_edge_kf),
+                       len(prob.line_edge_kf)))
+ba.bench_tries(15)
+ctx._check(lib.plp_ctx_kernel_timing(ctx.handle, 1))
+ba.bench_tries(30)
+buf = C.create_string_buffer(1 << 16)
+ctx._check(lib.plp_ctx_kernel_timing_report(ctx.handle, buf, C.c_size_t(len(buf))))
+ctx._check(lib.plp_ctx_kernel_timing(ctx.handle, 0))
+kt = json.loads(buf.value.decode())
+tot = sum(v["total_ms"] for v in kt.values())
+print(f"total {tot:.3f} ms for 31 tries -> {tot / 31 * 1e3:.1f} us/try")
+for k, v in sorted(kt.items(), key=lambda kv: -kv[1]["total_ms"]):
+    print(f"   {k:28s} n={v['count']:4d} mean_us={1e3 * v['total_ms'] / v['count']:8.1f} share={v['total_ms'] / tot:.3f}")
+ba.close()

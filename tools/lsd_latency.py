@@ -1,5 +1,6 @@
 """Latency of LSD + LBD extraction for small batches: one warp per frame vs the speculative multi-warp region growing
-(lines.cu lsd_grow_mw_kernel).  Run on the GPU box:  python tools/lsd_latency.py [warps ...]"""
+(lines.cu lsd_grow_mw_kernel) and the out-of-order one (lsd_grow_ooo_kernel).  Run on the GPU box:
+python tools/lsd_latency.py"""
 import ctypes as C
 import json
 import os
@@ -44,28 +45,21 @@ def kernel_ms(trk, imgs):
     return {k.split("<")[0].replace("_kernel", ""): round(v["total_ms"] / v["count"], 3) for k, v in kt.items()}
 
 
-# arguments: WARPS[:DIRECT] ...   (DIRECT = PLP_LSD_DIRECT bit mask: 1 multi-warp kernel, 2 one-warp kernel compute cos / sin)
-cfgs = [tuple(int(v) for v in a.split(":")) for a in sys.argv[1:]] or [(8,)]
-warps_list = [c[0] for c in cfgs]
-for cfg in cfgs:
-    warps = cfg[0]
-    os.environ["PLP_LSD_MW_WARPS"] = str(warps)
-    os.environ["PLP_LSD_DIRECT"] = str(cfg[1] if len(cfg) > 1 else 0)
-    for kind, fr in frames.items():
-        for batch in (1,):
-            imgs = np.concatenate([fr] * ((batch + 7) // 8))[:batch]
-            trk = plp.LineFeatureTracker(ctx, H, W, max_batch=batch)
-            out = {}
-            for variant in ((1, 2) if os.environ.get('PLP_TEST_OOO') == '0' else (1, 2, 3)):
-                trk.grow_variant(variant)
-                out[variant] = (timed(trk, imgs), kernel_ms(trk, imgs))
-                if variant == 2:
-                    st = trk.grow_stats(0)
-            st3 = trk.grow_stats(0, ooo=True)
-            n = len(trk.extract_batch(imgs)[0][0])
-            print(f"warps={warps} direct={os.environ['PLP_LSD_DIRECT']} {kind:8s} batch={batch:3d} keylines[0]={n:4d}  one-warp: {out[1][0]:7.2f} ms/call (grow {out[1][1].get('lsd_grow')})"
-                  f"   multi-warp: {out[2][0]:7.2f} ms/call (grow {out[2][1].get('lsd_grow_mw')})  stats {st}\n"
-                  + (f"          out-of-order: {out[3][0]:7.2f} ms/call (grow {out[3][1].get('lsd_grow_ooo')})  stats {st3}" if 3 in out else ""))
-            if batch == 1 and cfg == cfgs[0]:
-                print("    kernels (multi-warp run):", out[2][1])
-            trk.close()
+for kind, fr in frames.items():
+    for batch in (1,):
+        imgs = np.concatenate([fr] * ((batch + 7) // 8))[:batch]
+        trk = plp.LineFeatureTracker(ctx, H, W, max_batch=batch)
+        out = {}
+        for variant in ((1, 2) if os.environ.get('PLP_TEST_OOO') == '0' else (1, 2, 3)):
+            trk.grow_variant(variant)
+            out[variant] = (timed(trk, imgs), kernel_ms(trk, imgs))
+            if variant == 2:
+                st = trk.grow_stats(0)
+        st3 = trk.grow_stats(0, ooo=True)
+        n = len(trk.extract_batch(imgs)[0][0])
+        print(f"{kind:8s} batch={batch:3d} keylines[0]={n:4d}  one-warp: {out[1][0]:7.2f} ms/call (grow {out[1][1].get('lsd_grow')})"
+              f"   multi-warp: {out[2][0]:7.2f} ms/call (grow {out[2][1].get('lsd_grow_mw')})  stats {st}\n"
+              + (f"          out-of-order: {out[3][0]:7.2f} ms/call (grow {out[3][1].get('lsd_grow_ooo')})  stats {st3}" if 3 in out else ""))
+        if batch == 1 and kind == "plp":
+            print("    kernels (multi-warp run):", out[2][1])
+        trk.close()
