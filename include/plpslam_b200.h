@@ -288,6 +288,33 @@ PLP_API plp_status plp_undistort_keypoints_batch_dev(plp_ctx *ctx, const plp_cam
                                                      int batch, int cap, const plp_keypoint *d_kp, const int32_t *d_n_kp,
                                                      plp_keypoint *d_undist_out, double *d_bearings_out);
 
+/* util::stereo_rectifier (util/stereo_rectifier.cc:39-92): the StereoRectifier.* config keys and the rectified camera. */
+typedef struct plp_stereo_rectifier_params {
+    int32_t model;  /* StereoRectifier.model: 0 perspective, D = (k1, k2, p1, p2, k3); 1 fisheye, D = (k1, k2, k3, k4, -) */
+    double K_left[9], D_left[5], R_left[9];    /* row-major, as the config lists them */
+    double K_right[9], D_right[5], R_right[9];
+    double fx, fy, cx, cy; /* Camera.fx ... of the rectified camera (rounded to float, like cv_cam_matrix_) */
+} plp_stereo_rectifier_params;
+typedef struct plp_stereo_rectifier plp_stereo_rectifier;
+
+/* The constructor: both sides' maps (cv::initUndistortRectifyMap / cv::fisheye::initUndistortRectifyMap, CV_32F) for a
+ * rows x cols camera, kept on ctx's device.  PLP_ERR_INVALID for a model other than 0 / 1, a size <= 0 or a singular
+ * K_rect * R.  The rectifier may be used with any context on the same device. */
+PLP_API plp_status plp_stereo_rectifier_create(plp_ctx *ctx, const plp_stereo_rectifier_params *params, int rows, int cols,
+                                               plp_stereo_rectifier **out);
+PLP_API void plp_stereo_rectifier_destroy(plp_stereo_rectifier *r);
+/* stereo_rectifier::rectify: cv::remap(INTER_LINEAR, BORDER_CONSTANT 0) of both host images (rows x cols, row stride
+ * step) into left_out / right_out (row stride out_step).  Synchronous. */
+PLP_API plp_status plp_stereo_rectify(plp_ctx *ctx, const plp_stereo_rectifier *r, const uint8_t *left, const uint8_t *right,
+                                      size_t step, uint8_t *left_out, uint8_t *right_out, size_t out_step);
+/* Device-resident batch of one side (0 left, 1 right): frame b is read from d_in + b * rows * in_step and written to
+ * d_out + b * rows * out_step, only the first cols bytes of each row.  d_out and out_step must be multiples of 16, so d_out
+ * is a level 0 plp_orb_extract_batch_dev reads as it is.  Enqueued on ctx's stream, no synchronisation. */
+PLP_API plp_status plp_stereo_rectify_batch_dev(plp_ctx *ctx, const plp_stereo_rectifier *r, int side, const uint8_t *d_in,
+                                                int batch, size_t in_step, uint8_t *d_out, size_t out_step);
+/* The float maps of one side (host copies, rows x cols each). */
+PLP_API plp_status plp_stereo_rectifier_maps(const plp_stereo_rectifier *r, int side, float *map_x, float *map_y);
+
 typedef struct plp_image_view { /* one pyramid level, device memory */
     const uint8_t *data;
     int32_t rows, cols;

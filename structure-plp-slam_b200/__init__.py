@@ -12,6 +12,7 @@ from .capi import (  # noqa: F401
     OrbExtractor,
     LineFeatureTracker,
     BowVocabulary,
+    StereoRectifier,
     KP_DTYPE,
     KEYLINE_DTYPE,
     PT_OBS_DTYPE,

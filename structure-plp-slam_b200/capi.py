@@ -685,6 +685,80 @@ class BowVocabulary:
         return word[:n].copy(), node[:n].copy(), w[:n].copy()
 
 
+class StereoRectifierParams(C.Structure):
+    _fields_ = [("model", C.c_int32), ("K_left", C.c_double * 9), ("D_left", C.c_double * 5), ("R_left", C.c_double * 9),
+                ("K_right", C.c_double * 9), ("D_right", C.c_double * 5), ("R_right", C.c_double * 9),
+                ("fx", C.c_double), ("fy", C.c_double), ("cx", C.c_double), ("cy", C.c_double)]
+
+
+class StereoRectifier:
+    """util::stereo_rectifier backed by plp_stereo_rectifier: model 0 perspective (D = k1, k2, p1, p2, k3) or 1 fisheye
+    (D = k1..k4); K and R row-major 3x3 as the StereoRectifier.* config keys list them; (fx, fy, cx, cy) the rectified
+    camera."""
+
+    def __init__(self, ctx: Context, rows: int, cols: int, model, K_l, D_l, R_l, K_r, D_r, R_r, fx, fy, cx, cy):
+        self._ctx = ctx
+        self._lib = ctx._lib
+        self.rows, self.cols = int(rows), int(cols)
+
+        def arr(a, n):
+            v = np.asarray(a, np.float64).ravel()
+            if len(v) > n or (n == 9 and len(v) != 9):
+                raise PlpError(f"expected {n} values, got {len(v)}")
+            return (C.c_double * n)(*(list(v) + [0.0] * (n - len(v))))
+
+        self.params = StereoRectifierParams(int(model), arr(K_l, 9), arr(D_l, 5), arr(R_l, 9), arr(K_r, 9), arr(D_r, 5),
+                                            arr(R_r, 9), fx, fy, cx, cy)
+        h = C.c_void_p()
+        self._h = None
+        ctx._check(self._lib.plp_stereo_rectifier_create(ctx.handle, C.byref(self.params), C.c_int(rows), C.c_int(cols),
+                                                         C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if self._h is not None:
+            self._lib.plp_stereo_rectifier_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def handle(self):
+        return self._h
+
+    def rectify(self, left, right):
+        """stereo_rectifier::rectify of two host images -> (left_rect, right_rect)."""
+        left = np.ascontiguousarray(left, np.uint8)
+        right = np.ascontiguousarray(right, np.uint8)
+        if left.shape != (self.rows, self.cols) or right.shape != left.shape:
+            raise PlpError(f"images must be {self.rows} x {self.cols}")
+        out_l = np.zeros_like(left)
+        out_r = np.zeros_like(right)
+        self._ctx._check(self._lib.plp_stereo_rectify(self._ctx.handle, self._h, left.ctypes.data_as(_P),
+                                                      right.ctypes.data_as(_P), C.c_size_t(left.strides[0]),
+                                                      out_l.ctypes.data_as(_P), out_r.ctypes.data_as(_P),
+                                                      C.c_size_t(out_l.strides[0])))
+        return out_l, out_r
+
+    def rectify_dev(self, side, d_in, batch, in_step, d_out, out_step, ctx: Context = None):
+        """Device-resident batch of one side (device pointers), enqueued on ctx's stream (default: the creating one)."""
+        ctx = ctx or self._ctx
+        ctx._check(self._lib.plp_stereo_rectify_batch_dev(ctx.handle, self._h, C.c_int(side), d_in, C.c_int(batch),
+                                                          C.c_size_t(in_step), d_out, C.c_size_t(out_step)))
+
+    def maps(self, side):
+        """The float maps (map_x, map_y) of one side, rows x cols each."""
+        mx = np.zeros((self.rows, self.cols), np.float32)
+        my = np.zeros_like(mx)
+        self._ctx._check(self._lib.plp_stereo_rectifier_maps(self._h, C.c_int(side), mx.ctypes.data_as(_P),
+                                                             my.ctypes.data_as(_P)))
+        return mx, my
+
+
 def fold_bow(word_id, node_id, weight):
     """The adapter's fold of transform() rows into DBoW2's two maps (TemplatedVocabulary::transform(features, v, fv,
     levelsup) with TF_IDF weighting and L1 scoring): rows with weight > 0 only; bow_vec[word] += weight in row order,

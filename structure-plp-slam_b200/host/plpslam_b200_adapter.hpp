@@ -23,9 +23,11 @@
 #include <cstring>
 #include <set>
 #include <stdexcept>
+#include <string>
 #include <vector>
 
 #include <opencv2/core.hpp>
+#include <opencv2/core/mat.hpp>
 
 #include "PLPSLAM/camera/perspective.h"
 #include "PLPSLAM/data/frame.h"
@@ -85,6 +87,40 @@ inline void undistort_keypoints(const plp_camera &cam, const plp_distortion &dis
     bearings.resize(n);
     for (int i = 0; i < n; ++i) bearings[i] = PLPSLAM::Vec3_t{b[3 * i], b[3 * i + 1], b[3 * i + 2]};
 }
+
+// ---- util::stereo_rectifier (util/stereo_rectifier.cc:39-92) ----------------------------------------------
+// The constructor fills plp_stereo_rectifier_params from the StereoRectifier.* keys and the camera's fx_, fy_, cx_, cy_
+// (see INTEGRATION.md) and calls create(); rectify() replaces the two cv::remap calls.  The GPU rectifies 8-bit
+// single-channel images of the camera's size.  cv::remap would take any type and size, so anything else (a BGR frame of
+// cv::VideoCapture, an image of another size) is rejected here instead of being read as a gray image of the camera's size.
+struct stereo_rectifier_backend {
+    plp_stereo_rectifier *h = nullptr;
+    int rows = 0, cols = 0;
+    stereo_rectifier_backend() = default;
+    stereo_rectifier_backend(const stereo_rectifier_backend &) = delete;
+    stereo_rectifier_backend &operator=(const stereo_rectifier_backend &) = delete;
+    ~stereo_rectifier_backend() { plp_stereo_rectifier_destroy(h); }
+    void create(const plp_stereo_rectifier_params &p, int r, int c) {
+        check(plp_stereo_rectifier_create(thread_ctx(), &p, r, c, &h));
+        rows = r;
+        cols = c;
+    }
+    void require_gray_of_camera_size(const cv::Mat &m, const char *side) const {
+        if (m.empty() || cv::_InputArray(m).type() != CV_8UC1 || m.rows != rows || m.cols != cols)
+            throw std::runtime_error(std::string("plpslam_b200: stereo_rectifier::rectify: the ") + side +
+                                     " image must be 8-bit single-channel (CV_8UC1) of " + std::to_string(rows) + " x " +
+                                     std::to_string(cols) + " (convert colour frames to gray before rectifying)");
+    }
+    void rectify(const cv::Mat &in_l, const cv::Mat &in_r, cv::Mat &out_l, cv::Mat &out_r) const {
+        require_gray_of_camera_size(in_l, "left");
+        require_gray_of_camera_size(in_r, "right");
+        if (in_l.step != in_r.step) throw std::runtime_error("plpslam_b200: left and right images differ in row stride");
+        out_l.create(rows, cols, CV_8UC1);
+        out_r.create(rows, cols, CV_8UC1);
+        if (out_l.step != out_r.step) throw std::runtime_error("plpslam_b200: output images differ in row stride");
+        check(plp_stereo_rectify(thread_ctx(), h, in_l.data, in_r.data, in_l.step, out_l.data, out_r.data, out_l.step));
+    }
+};
 
 // ---- feature::orb_extractor::extract (feature/orb_extractor.cc:73-160) -------------------------------------
 struct orb_backend {

@@ -10,9 +10,12 @@ line_extract.npz    LineFeatureTracker::extract_LSD_LBD output of the oracle (wh
 cv2_lsd_odd.npz     cv2's half-resolution LSD image and LSD segments at sizes with a dimension = 3 (mod 4)
 cv2_undistort.npz   cv2.undistortPointsIter / cv2.fisheye.undistortPoints of seeded points for every camera of
                     tests/camera_data.py, with the oracle's undistortion and image bounds beside them
+cv2_rectify.npz     cv2.initUndistortRectifyMap / cv2.fisheye.initUndistortRectifyMap (CV_32F) of every rectifier of
+                    tests/rectify_data.py: 4000 seeded pixels and the SHA-256 of the full maps per side; cv2.remap
+                    (INTER_LINEAR) of a seeded texture through the EuRoC and TUM-VI left maps and through random maps
 The images are regenerated from their seeds by the tests; only the outputs are stored.
 
-    python tools/gen_golden.py cv2_lsd_odd cv2_undistort      # only the named files"""
+    python tools/gen_golden.py cv2_lsd_odd cv2_undistort cv2_rectify      # only the named files"""
 import sys
 from pathlib import Path
 
@@ -26,6 +29,7 @@ import synth  # noqa: E402
 import test_golden  # noqa: E402
 import test_orb_oracle  # noqa: E402
 import camera_data  # noqa: E402
+import rectify_data  # noqa: E402
 
 OUT = ROOT / "tests" / "golden"
 
@@ -54,11 +58,32 @@ def undistort():
     np.savez_compressed(OUT / "cv2_undistort.npz", **out)
 
 
+def rectify():
+    import hashlib
+    rd = rectify_data
+    out = {}
+    for case, c in rd.CASES.items():
+        rng = np.random.default_rng(17)
+        idx = rng.integers(0, c["rows"] * c["cols"], 4000).astype(np.int32)
+        out[case + "_idx"] = idx
+        for side in (0, 1):
+            mx, my = rd.cv2_maps(case, side)
+            key = f"{case}_{side}"
+            out[key + "_x"], out[key + "_y"] = mx.ravel()[idx], my.ravel()[idx]
+            out[key + "_sha256"] = np.array(hashlib.sha256(mx.tobytes() + my.tobytes()).hexdigest())
+            if side == 0 and case in rd.REFERENCE_CASES:
+                out[case + "_remap"] = cv2.remap(rd.texture(23, c["rows"], c["cols"]), mx, my, cv2.INTER_LINEAR)
+    mx, my = rd.random_maps(1, 200, 300, 97, 131)
+    out["random_remap"] = cv2.remap(rd.texture(5, 97, 131), mx, my, cv2.INTER_LINEAR)
+    out["cv2_version"] = np.array(cv2.__version__)
+    np.savez_compressed(OUT / "cv2_rectify.npz", **out)
+
+
 def main():
     OUT.mkdir(exist_ok=True)
     if sys.argv[1:]:
         for name in sys.argv[1:]:
-            {"cv2_lsd_odd": lsd_odd, "cv2_undistort": undistort}[name]()
+            {"cv2_lsd_odd": lsd_odd, "cv2_undistort": undistort, "cv2_rectify": rectify}[name]()
         return
     orc = oracle_api.Oracle()
     tex = synth.make_texture(4321, 240, 320, n_rect=120, n_blob=500)      # the image of __graft_entry__.smoke()
@@ -96,6 +121,7 @@ def main():
     np.savez_compressed(OUT / "line_extract.npz", keylines=kl, lbd=lbd, line_functions=fn)
     lsd_odd()
     undistort()
+    rectify()
     for f in sorted(OUT.glob("*.npz")):
         print(f.name, f.stat().st_size, "bytes")
 
