@@ -6,13 +6,12 @@
 
 #include "../../include/plpslam_b200.h"
 #include "devmath.cuh"
+#include "match_common.cuh"
 
 namespace plp {
 
 namespace {
 
-constexpr int kHistLen = 30;    // angle_checker.h:47
-constexpr int kNumBinsThr = 3;  // angle_checker.h:48
 constexpr int kMatchThreads = 256;
 
 struct VocabDev {
@@ -22,12 +21,6 @@ struct VocabDev {
     const float *weight;
     const int32_t *word_id;
 };
-
-__device__ __forceinline__ void load_desc(const uint8_t *p, uint4 &a, uint4 &b) {
-    const uint4 *q = reinterpret_cast<const uint4 *>(p);
-    a = __ldg(q);
-    b = __ldg(q + 1);
-}
 
 // TemplatedVocabulary::transform(feature, word_id, weight, &nid, levelsup)
 template <int G>
@@ -51,11 +44,7 @@ __global__ void __launch_bounds__(256) bow_transform_kernel(VocabDev V, const ui
             const unsigned long long key = ((unsigned long long)(unsigned)hamming256(q0, q1, d0, d1) << 32) | (c - beg);
             best = key < best ? key : best;
         }
-#pragma unroll
-        for (int o = G / 2; o > 0; o >>= 1) {
-            const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
-            best = other < best ? other : best;
-        }
+        best = warp_min<G>(best);
         if (beg < end) {
             ++level;
             final_id = (int)V.children[beg + (uint32_t)(best & 0xffffffffull)];
@@ -88,37 +77,10 @@ struct BowJob {
     uint32_t *num_matches;
 };
 
-// angle_checker.h:100-113
-__device__ __forceinline__ int angle_bin(float delta_angle) {
-    if (delta_angle < 0.0) delta_angle = (float)((double)delta_angle + 360.0);
-    if (360.0 <= delta_angle) delta_angle = (float)((double)delta_angle - 360.0);
-    const float inv_len = 1.0f / (float)kHistLen;
-    return __float2int_rn(delta_angle * inv_len);
-}
-
-// angle_checker.h:163-175 with the oracle's stable ranking (size desc, bin index asc); one thread
-__device__ void rank_bins(const int *hist, uint8_t *bin_valid) {
-    bool used[kHistLen];
-    for (int b = 0; b < kHistLen; ++b) {
-        used[b] = false;
-        bin_valid[b] = 0;
-    }
-    for (int k = 0; k < kNumBinsThr; ++k) {
-        int best = -1, best_cnt = -1;
-        for (int b = 0; b < kHistLen; ++b)
-            if (!used[b] && hist[b] > best_cnt) {
-                best_cnt = hist[b];
-                best = b;
-            }
-        used[best] = true;
-        bin_valid[best] = 1;
-    }
-}
-
 __global__ void __launch_bounds__(kMatchThreads) bow_match_kernel(const BowJob *__restrict__ jobs, float lowe_ratio,
                                                                   int check_orientation) {
-    __shared__ int s_hist[kHistLen + 2];
-    __shared__ uint8_t s_bin_valid[kHistLen + 2];
+    __shared__ int s_hist[kHistLen];
+    __shared__ uint8_t s_bin_valid[kHistLen];
     __shared__ int s_cnt[2];
     const BowJob &J = jobs[blockIdx.x];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = kMatchThreads / 32;
@@ -128,7 +90,7 @@ __global__ void __launch_bounds__(kMatchThreads) bow_match_kernel(const BowJob *
         J.claimed[j] = 0;
         J.matched_1_of_2[j] = -1;
     }
-    for (int b = tid; b < kHistLen + 2; b += kMatchThreads) s_hist[b] = 0;
+    for (int b = tid; b < kHistLen; b += kMatchThreads) s_hist[b] = 0;
     if (tid < 2) s_cnt[tid] = 0;
     __syncthreads();
     for (int node = warp; node < J.num_nodes; node += nwarps) {
@@ -155,15 +117,7 @@ __global__ void __launch_bounds__(kMatchThreads) bow_match_kernel(const BowJob *
                     k2 = key;
                 }
             }
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) {
-                const unsigned long long o1 = __shfl_xor_sync(0xffffffffu, k1, o);
-                const unsigned long long o2 = __shfl_xor_sync(0xffffffffu, k2, o);
-                const unsigned long long lo = k1 < o1 ? k1 : o1, hi = k1 < o1 ? o1 : k1;
-                const unsigned long long s2 = k2 < o2 ? k2 : o2;
-                k1 = lo;
-                k2 = hi < s2 ? hi : s2;
-            }
+            warp_top2<32>(k1, k2);
             if (k1 != ~0ull) {
                 const unsigned best = (unsigned)(k1 >> 32);
                 const unsigned second = k2 != ~0ull ? (unsigned)(k2 >> 32) : (unsigned)PLP_MAX_HAMMING_DIST;
@@ -182,27 +136,13 @@ __global__ void __launch_bounds__(kMatchThreads) bow_match_kernel(const BowJob *
     __syncthreads();
     // orientation histogram (:123-127, :152-160) and outputs
     const bool do_angle = check_orientation && J.angle1 && J.angle2;
-    for (int i = tid; i < J.n1; i += kMatchThreads) {
-        const int j = J.choice[i];
-        if (j < 0) continue;
-        atomicAdd(&s_cnt[0], 1);
-        if (do_angle) atomicAdd(&s_hist[angle_bin(J.angle1[i] - J.angle2[j])], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-        if (do_angle)
-            rank_bins(s_hist, s_bin_valid);
-        else
-            for (int b = 0; b < kHistLen + 2; ++b) s_bin_valid[b] = 1;
-    }
-    __syncthreads();
+    const auto delta = [&](int i, int j) { return J.angle1[i] - J.angle2[j]; };
+    orientation_check<kMatchThreads>(J.n1, J.choice, do_angle, s_hist, s_bin_valid, &s_cnt[0], delta);
     for (int i = tid; i < J.n1; i += kMatchThreads) {
         const int j = J.choice[i];
         int out = -1;
         if (j >= 0) {
-            bool keep = true;
-            if (do_angle) keep = s_bin_valid[angle_bin(J.angle1[i] - J.angle2[j])] != 0;
-            if (keep) {
+            if (!do_angle || s_bin_valid[angle_bin(delta(i, j))]) {
                 out = j;
                 J.matched_1_of_2[j] = i;
             } else {

@@ -9,8 +9,8 @@
 // Exactness: reprojection, the distance / viewing-angle gates and the chi-square gates are evaluated in the reference's
 // double / float mix (this file is compiled with -fmad=false); predict_scale_level's logf becomes a comparison of the
 // float ratio against thresholds derived on the host from the caller's own libm (see build_level_thresholds);
-// candidates are visited in get_keypoints_in_cell order (cell-x, cell-y, insertion) via the same rank sort as match.cu,
-// and "first strictly smaller distance wins" is min(distance << 32 | traversal position).
+// candidates are visited in get_keypoints_in_cell order (cell-x, cell-y, insertion) via the cell sort the window matcher
+// uses (match_common.cuh), and "first strictly smaller distance wins" is min(distance << 32 | traversal position).
 #include "common.cuh"
 #include "pack.cuh"
 #include "fuse_kernels.cuh"

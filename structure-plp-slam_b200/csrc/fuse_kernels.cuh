@@ -7,6 +7,7 @@
 
 #include "../../include/plpslam_b200.h"
 #include "devmath.cuh"
+#include "match_common.cuh"
 
 namespace plp {
 
@@ -23,7 +24,7 @@ struct FusePointTarget {
     const int32_t *octave;
     const uint8_t *desc;
     const uint8_t *skip;  // may be null
-    double R[9], t[3], c[3];
+    double R[9], t[3], c[3];  // the layout of plp_fuse_target_*: rot_cw, trans_cw, cam_center
 };
 
 struct FuseLineTarget {
@@ -55,12 +56,6 @@ struct FuseParams {
     int mode;
 };
 
-__device__ __forceinline__ void load_desc(const uint8_t *p, uint4 &a, uint4 &b) {
-    const uint4 *q = reinterpret_cast<const uint4 *>(p);
-    a = __ldg(q);
-    b = __ldg(q + 1);
-}
-
 // data/landmark.cc:341-362 through the host-derived threshold table
 __device__ __forceinline__ int predict_level(float ratio, const FuseParams &P) {
     int lvl = 0;
@@ -68,38 +63,15 @@ __device__ __forceinline__ int predict_level(float ratio, const FuseParams &P) {
     return lvl;
 }
 
-struct Proj {
-    double u, v;
-    float x_right;
-    bool in_image;
-};
-
-// camera/perspective.cc:190-209; a point behind the camera leaves (u, v) = (0, 0) (the reference leaves them unset)
-__device__ __forceinline__ Proj reproject(const plp_camera &cam, const double *R, const double *t, const double *X) {
-    Proj r;
-    r.u = 0.0;
-    r.v = 0.0;
-    r.x_right = 0.0f;
-    r.in_image = false;
-    const double pc0 = R[0] * X[0] + R[1] * X[1] + R[2] * X[2] + t[0];
-    const double pc1 = R[3] * X[0] + R[4] * X[1] + R[5] * X[2] + t[1];
-    const double pc2 = R[6] * X[0] + R[7] * X[1] + R[8] * X[2] + t[2];
-    if (pc2 <= 0.0) return r;
-    const double z_inv = 1.0 / pc2;
-    r.u = cam.fx * pc0 * z_inv + cam.cx;
-    r.v = cam.fy * pc1 * z_inv + cam.cy;
-    r.x_right = (float)(r.u - cam.focal_x_baseline * z_inv);
-    r.in_image = (cam.min_x < r.u && r.u < cam.max_x && cam.min_y < r.v && r.v < cam.max_y);
-    return r;
-}
-
-__device__ __forceinline__ unsigned long long warp_min_u64(unsigned long long k) {
+// the rows of [R | t], the pose layout reproject() takes
+__device__ __forceinline__ void pose_rows(const double *R, const double *t, double *Rt) {
 #pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long other = __shfl_xor_sync(0xffffffffu, k, o);
-        k = other < k ? other : k;
+    for (int r = 0; r < 3; ++r) {
+        Rt[4 * r] = R[3 * r];
+        Rt[4 * r + 1] = R[3 * r + 1];
+        Rt[4 * r + 2] = R[3 * r + 2];
+        Rt[4 * r + 3] = t[r];
     }
-    return k;
 }
 
 static size_t fuse_point_smem_bytes(int cap, int cells) {
@@ -144,78 +116,9 @@ __global__ void __launch_bounds__(kThreads, 1)
     base += (size_t)(cells + 2) * 4;
     int *s_warp = reinterpret_cast<int *>(base);
 
-    // ---- 1. cell key of every keypoint (data/common.h:104-109) and the cell histogram
-    for (int k = tid; k < cells + 2; k += kThreads) s_cell_start[k] = 0;
-    __syncthreads();
-    for (int i = tid; i < n; i += kThreads) {
-        const float px = T.x[i], py = T.y[i];
-        const int cx = cv_floor((double)(px - grid.min_x) * grid.inv_cell_width);
-        const int cy = cv_floor((double)(py - grid.min_y) * grid.inv_cell_height);
-        const bool in = (0 <= cx && cx < grid.num_cols && 0 <= cy && cy < grid.num_rows);
-        const int key = in ? cx * grid.num_rows + cy : cells;  // out-of-grid keypoints sort last and are never visited
-        s_key[i] = key;
-        atomicAdd(&s_cell_start[key], 1);
-    }
-    __syncthreads();
-    // ---- 2. stable counting sort by (cell key, index) = traversal order of get_keypoints_in_cell
-    //         (data/common.cc:275-309).  (a) exclusive scan of the histogram: cell_start[k] = first sorted position
-    //         whose key >= k; (b) one warp walks the keypoints in index order, __match_any groups equal keys and gives
-    //         every lane its rank inside the group, the group leader advances the cell cursor.
-    {
-        const int total = cells + 1;  // keys 0 .. cells
-        const int per = (total + kThreads - 1) / kThreads;
-        const int b0 = min(total, tid * per), b1 = min(total, b0 + per);
-        int sum = 0;
-        for (int k = b0; k < b1; ++k) sum += s_cell_start[k];
-        int incl = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += v;
-        }
-        if (lane == 31) s_warp[warp] = incl;
-        __syncthreads();
-        if (warp == 0) {
-            const int v = lane < nwarps ? s_warp[lane] : 0;
-            int sc = v;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int u = __shfl_up_sync(0xffffffffu, sc, o);
-                if (lane >= o) sc += u;
-            }
-            if (lane < nwarps) s_warp[lane] = sc - v;  // exclusive prefix of the warp totals
-        }
-        __syncthreads();
-        int run = s_warp[warp] + incl - sum;
-        for (int k = b0; k < b1; ++k) {
-            const int v = s_cell_start[k];
-            s_cell_start[k] = run;
-            s_cursor[k] = run;
-            run += v;
-        }
-        if (tid == 0) s_cell_start[cells + 1] = n;
-        __syncthreads();
-        if (warp == 0) {
-            for (int base = 0; base < n; base += 32) {
-                const int i = base + lane;
-                const int key = i < n ? s_key[i] : (0x40000000 | lane);  // idle lanes get unique keys
-                const unsigned peers = __match_any_sync(0xffffffffu, key);
-                const int leader = __ffs(peers) - 1;
-                const int rank = __popc(peers & ((1u << lane) - 1));
-                int b = 0;
-                if (lane == leader && i < n) {
-                    b = s_cursor[key];
-                    s_cursor[key] = b + __popc(peers);
-                }
-                b = __shfl_sync(0xffffffffu, b, leader);
-                if (i < n) s_orig[b + rank] = i;
-                __syncwarp();
-            }
-        }
-    }
-    __syncthreads();
-    const int n_in = s_cell_start[cells];
-    // ---- 3. gather in sorted order; s_oct keeps the octave, the cell key is re-read from s_key through s_orig
+    // ---- 1-2. stable sort by (cell key, index) = traversal order of get_keypoints_in_cell
+    const int n_in = sort_by_cell<kThreads>(grid, n, T.x, T.y, s_key, s_cell_start, s_cursor, s_warp, s_orig);
+    // ---- 3. gather in sorted order
     for (int p = tid; p < n_in; p += kThreads) {
         const int i = s_orig[p];
         s_x[p] = T.x[i];
@@ -239,7 +142,9 @@ __global__ void __launch_bounds__(kThreads, 1)
         unsigned pred = 0;
         if (ok) {
             const double X[3] = {L.pos_w[3 * (size_t)i], L.pos_w[3 * (size_t)i + 1], L.pos_w[3 * (size_t)i + 2]};
-            const Proj pr = reproject(P.cam, T.R, T.t, X);
+            double Rt[12];
+            pose_rows(T.R, T.t, Rt);
+            const Reproj pr = reproject(P.cam, Rt, X);
             ok = pr.in_image;
             u = pr.u;
             v = pr.v;
@@ -256,19 +161,15 @@ __global__ void __launch_bounds__(kThreads, 1)
         }
         if (ok && n_in > 0) {
             const float ref_x = (float)u, ref_y = (float)v, r = P.margin * P.scale_factors[pred];
-            // data/common.cc:249-272
-            const int min_cx = max(0, cv_floor((double)(ref_x - grid.min_x - r) * grid.inv_cell_width));
-            const int max_cx = min(grid.num_cols - 1, cv_ceil((double)(ref_x - grid.min_x + r) * grid.inv_cell_width));
-            const int min_cy = max(0, cv_floor((double)(ref_y - grid.min_y - r) * grid.inv_cell_height));
-            const int max_cy = min(grid.num_rows - 1, cv_ceil((double)(ref_y - grid.min_y + r) * grid.inv_cell_height));
+            Window w;
             unsigned long long best = ~0ull;
-            if (min_cx < grid.num_cols && max_cx >= 0 && min_cy < grid.num_rows && max_cy >= 0) {
+            if (query_window(grid, ref_x, ref_y, r, w)) {
                 uint4 q0, q1;
                 load_desc(L.desc + 32 * (size_t)i, q0, q1);
                 const int pred_i = (int)pred;
-                for (int c = min_cx; c <= max_cx; ++c) {
-                    const int p_begin = s_cell_start[c * grid.num_rows + min_cy];
-                    const int p_end = s_cell_start[c * grid.num_rows + max_cy + 1];
+                for (int c = w.min_cx; c <= w.max_cx; ++c) {
+                    const int p_begin = s_cell_start[c * grid.num_rows + w.min_cy];
+                    const int p_end = s_cell_start[c * grid.num_rows + w.max_cy + 1];
                     for (int p = p_begin + lane; p < p_end; p += 32) {
                         const float kx = s_x[p], ky = s_y[p];
                         const float dx = kx - ref_x, dy = ky - ref_y;
@@ -297,7 +198,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                     }
                 }
             }
-            best = warp_min_u64(best);
+            best = warp_min<32>(best);
             if (best != ~0ull) {
                 const unsigned d = (unsigned)(best >> 32);
                 // best_dist starts at MAX_HAMMING_DIST with a strict '<' (:221-276), then HAMMING_DIST_THR_LOW (:279-282)
@@ -362,7 +263,9 @@ __global__ void __launch_bounds__(kThreads, 1)
         if (ok) {
             const double *pw = L.pos_w + 6 * (size_t)i;
             const double S[3] = {pw[0], pw[1], pw[2]}, E[3] = {pw[3], pw[4], pw[5]};
-            const Proj ps = reproject(P.cam, T.R, T.t, S), pe = reproject(P.cam, T.R, T.t, E);
+            double Rt[12];
+            pose_rows(T.R, T.t, Rt);
+            const Reproj ps = reproject(P.cam, Rt, S), pe = reproject(P.cam, Rt, E);
             su = ps.u;
             sv = ps.v;
             eu = pe.u;
@@ -370,7 +273,7 @@ __global__ void __launch_bounds__(kThreads, 1)
             if (!ps.in_image && !pe.in_image) ok = false;  // :341-345
             const double M[3] = {0.5 * (S[0] + E[0]), 0.5 * (S[1] + E[1]), 0.5 * (S[2] + E[2])};
             if (ok && (!ps.in_image || !pe.in_image)) {  // :347-366
-                const Proj pm = reproject(P.cam, T.R, T.t, M);
+                const Reproj pm = reproject(P.cam, Rt, M);
                 if (!pm.in_image) ok = false;
             }
             if (ok) {  // :368-392
@@ -410,7 +313,7 @@ __global__ void __launch_bounds__(kThreads, 1)
                 const unsigned long long key = ((unsigned long long)d << 32) | (unsigned)p;
                 best = key < best ? key : best;
             }
-            best = warp_min_u64(best);
+            best = warp_min<32>(best);
             if (best != ~0ull) {
                 const unsigned d = (unsigned)(best >> 32);
                 if (d < (unsigned)PLP_MAX_HAMMING_DIST && d <= (unsigned)PLP_HAMMING_DIST_THR_LOW) {

@@ -16,6 +16,7 @@
 // 2 x uint4; distances are 8 x __popc.
 //
 // Compiled with -fmad=false: float/double expressions must round exactly like the oracle.
+#include "match_common.cuh"
 #include "match_kernels.cuh"
 #include "point_match_kernels.cuh"
 #include "detmath.h"
@@ -26,43 +27,6 @@ namespace plp {
 namespace {
 
 constexpr int kThreads = 512;
-constexpr int kHistLen = 30;     // angle_checker.h:47
-constexpr int kNumBinsThr = 3;   // angle_checker.h:48
-
-// angle_checker.h:100-113
-__device__ __forceinline__ int angle_bin(float delta_angle) {
-    if (delta_angle < 0.0) delta_angle = (float)((double)delta_angle + 360.0);
-    if (360.0 <= delta_angle) delta_angle = (float)((double)delta_angle - 360.0);
-    const float inv_len = 1.0f / (float)kHistLen;
-    return __float2int_rn(delta_angle * inv_len);
-}
-
-// angle_checker.h:163-175: rank bins by size (desc), ties by bin index (asc); first 3 are valid.
-// Executed by one thread; hist/valid in shared memory.
-__device__ void rank_bins(const int *hist, uint8_t *bin_valid) {
-    bool used[kHistLen];
-    for (int b = 0; b < kHistLen; ++b) {
-        used[b] = false;
-        bin_valid[b] = 0;
-    }
-    for (int k = 0; k < kNumBinsThr; ++k) {
-        int best = -1, best_cnt = -1;
-        for (int b = 0; b < kHistLen; ++b)
-            if (!used[b] && hist[b] > best_cnt) {
-                best_cnt = hist[b];
-                best = b;
-            }
-        used[best] = true;
-        bin_valid[best] = 1;
-    }
-}
-
-__device__ __forceinline__ void load_desc(const uint8_t *p, uint4 &a, uint4 &b) {
-    const uint4 *q = reinterpret_cast<const uint4 *>(p);
-    a = __ldg(q);
-    b = __ldg(q + 1);
-}
-
 // ---------------------------------------------------------------------------------------
 // dense Hamming matrix and exact 1-NN
 // ---------------------------------------------------------------------------------------
@@ -98,11 +62,7 @@ __global__ void hamming_nn_kernel(const uint8_t *__restrict__ q, int nq, const u
         const unsigned long long key = ((unsigned long long)hamming256(q0, q1, t0, t1) << 32) | (unsigned)j;
         best = key < best ? key : best;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) {
-        const unsigned long long other = __shfl_xor_sync(0xffffffffu, best, o);
-        best = other < best ? other : best;
-    }
+    best = warp_min<32>(best);
     if (lane == 0) {
         nn_idx[warp] = nt > 0 ? (int32_t)(best & 0xffffffffu) : -1;
         nn_dist[warp] = nt > 0 ? (uint16_t)(best >> 32) : (uint16_t)0xFFFF;
@@ -112,33 +72,6 @@ __global__ void hamming_nn_kernel(const uint8_t *__restrict__ q, int nq, const u
 // ---------------------------------------------------------------------------------------
 // reprojection pre-pass of match_current_and_last_frames (projection.cc:240-292)
 // ---------------------------------------------------------------------------------------
-struct Reproj {
-    double u, v;
-    float x_right;
-    bool in_image;
-    bool in_front;
-};
-
-// camera/perspective.cc:190-209
-__device__ __forceinline__ Reproj reproject(const plp_camera &cam, const double *P, const double *X) {
-    Reproj r;
-    const double pc0 = P[0] * X[0] + P[1] * X[1] + P[2] * X[2] + P[3];
-    const double pc1 = P[4] * X[0] + P[5] * X[1] + P[6] * X[2] + P[7];
-    const double pc2 = P[8] * X[0] + P[9] * X[1] + P[10] * X[2] + P[11];
-    r.u = 0.0;
-    r.v = 0.0;
-    r.x_right = 0.0f;
-    r.in_image = false;
-    r.in_front = pc2 > 0.0;
-    if (!r.in_front) return r;
-    const double z_inv = 1.0 / pc2;
-    r.u = cam.fx * pc0 * z_inv + cam.cx;
-    r.v = cam.fy * pc1 * z_inv + cam.cy;
-    r.x_right = (float)(r.u - cam.focal_x_baseline * z_inv);
-    r.in_image = (cam.min_x < r.u && r.u < cam.max_x && cam.min_y < r.v && r.v < cam.max_y);
-    return r;
-}
-
 __global__ void project_points_kernel(const ProjectJob *__restrict__ jobs, plp_camera cam,
                                       const float *__restrict__ scale_factors, int num_levels, float margin) {
     const ProjectJob &J = jobs[blockIdx.y];
@@ -208,6 +141,38 @@ __global__ void project_lines_kernel(const ProjectJob *__restrict__ jobs, plp_ca
     J.qvalid[i] = valid ? 1 : 0;
 }
 
+// The sequential greedy "query q takes its best candidate not claimed by a query < q" of the round-based matchers,
+// iterated to its fixed point (see the top of this file).  Called by every thread of the CTA.  choose(q, owner) is query
+// q's candidate given the claims `owner` of the previous round (owner[c] < q: c is taken), or -1.  On entry owner_prev
+// and owner_next hold kNoOwner for the n candidates and *flag is 0, visible to every thread; on return choice[0, m) is
+// the sequential result.  `choice` is the job's own pointer, taken by reference so that the kernels re-read it rather
+// than hold it in two more registers through the candidate scans.
+template <class Choose>
+__device__ __forceinline__ void claim_fixed_point(int m, int n, int *owner_prev, int *owner_next, int *flag,
+                                                  int32_t *const &choice, Choose choose) {
+    const int tid = threadIdx.x;
+    for (int round = 0; round <= m; ++round) {
+        for (int q = tid; q < m; q += kThreads) {
+            const int c = choose(q, owner_prev);
+            choice[q] = c;
+            if (c >= 0) atomicMin(&owner_next[c], q);
+        }
+        __syncthreads();
+        for (int p = tid; p < n; p += kThreads)
+            if (owner_next[p] != owner_prev[p]) *flag = 1;
+        __syncthreads();
+        const int changed = *flag;
+        __syncthreads();
+        if (!changed) break;
+        if (tid == 0) *flag = 0;
+        int *t = owner_prev;
+        owner_prev = owner_next;
+        owner_next = t;
+        for (int p = tid; p < n; p += kThreads) owner_next[p] = kNoOwner;
+        __syncthreads();
+    }
+}
+
 // ---------------------------------------------------------------------------------------
 // keyline matcher: candidates = linear scan (data/common.cc:315-364)
 // ---------------------------------------------------------------------------------------
@@ -221,85 +186,69 @@ __global__ void __launch_bounds__(kThreads, 1)
     int *owner_next = owner_prev + n;
     int *flags = owner_next + n;
     for (int p = tid; p < n; p += kThreads) {
-        owner_prev[p] = 0x7fffffff;
-        owner_next[p] = 0x7fffffff;
+        owner_prev[p] = kNoOwner;
+        owner_next[p] = kNoOwner;
     }
     if (tid < 4) flags[tid] = 0;
     __syncthreads();
-    for (int round = 0; round <= m; ++round) {
-        for (int q = tid; q < m; q += kThreads) {
-            int choice = -1;
-            const bool valid = J.qvalid ? (J.qvalid[q] != 0) : true;
-            if (valid) {
-                const float margin = J.qradius[q];
-                const int min_level = J.qmin[q], max_level = J.qmax[q];
-                const bool check_level = (0 < min_level) || (0 <= max_level);
-                // proj_line = (x1,y1,1) x (x2,y2,1) in double (data/common.cc:325-327)
-                const double ax = J.q_spx[q], ay = J.q_spy[q], bx = J.q_epx[q], by = J.q_epy[q];
-                const double l0 = ay * 1.0 - 1.0 * by;
-                const double l1 = 1.0 * bx - ax * 1.0;
-                const double l2 = ax * by - ay * bx;
-                const double den = sqrt(l0 * l0 + l1 * l1);
-                uint4 q0, q1;
-                load_desc(J.qdesc + 32 * (size_t)q, q0, q1);
-                unsigned best = PLP_MAX_HAMMING_DIST, second = PLP_MAX_HAMMING_DIST;
-                int best_lvl = -1, second_lvl = -1, best_p = -1;
-                for (int p = 0; p < n; ++p) {
-                    const float dsp = (float)((J.sx[p] * l0 + J.sy[p] * l1 + l2) / den);
-                    const float dep = (float)((J.ex[p] * l0 + J.ey[p] * l1 + l2) / den);
-                    if (fabsf(dsp) > margin || fabsf(dep) > margin) continue;
-                    if (check_level) {
-                        const int oct = J.octave[p];
-                        if (oct < min_level) continue;
-                        if (max_level > 0 && oct > max_level) continue;
-                    }
-                    if (J.claimed && J.claimed[p]) continue;
-                    if (owner_prev[p] < q) continue;
-                    if (rgbd_gate && J.xr_sp && J.xr_ep && J.q_xr_sp && J.q_xr_ep) {  // projection.cc:487-500
-                        if (J.xr_sp[p] > 0 && J.xr_ep[p] > 0) {
-                            const float e_sp = fabsf(J.q_xr_sp[q] - J.xr_sp[p]);
-                            const float e_ep = fabsf(J.q_xr_ep[q] - J.xr_ep[p]);
-                            if (margin < e_sp || margin < e_ep) continue;
-                        }
-                    }
-                    uint4 d0, d1;
-                    load_desc(J.desc + 32 * (size_t)p, d0, d1);
-                    const unsigned d = (unsigned)hamming256(q0, q1, d0, d1);
-                    const int lvl = J.ratio_level ? J.ratio_level[p] : J.octave[p];
-                    if (d < best) {
-                        second = best;
-                        best = d;
-                        second_lvl = best_lvl;
-                        best_lvl = lvl;
-                        best_p = p;
-                    } else if (d < second) {
-                        second_lvl = lvl;
-                        second = d;
+    claim_fixed_point(m, n, owner_prev, owner_next, &flags[0], J.choice, [&](int q, const int *owner) {
+        int choice = -1;
+        const bool valid = J.qvalid ? (J.qvalid[q] != 0) : true;
+        if (valid) {
+            const float margin = J.qradius[q];
+            const int min_level = J.qmin[q], max_level = J.qmax[q];
+            const bool check_level = (0 < min_level) || (0 <= max_level);
+            // proj_line = (x1,y1,1) x (x2,y2,1) in double (data/common.cc:325-327)
+            const double ax = J.q_spx[q], ay = J.q_spy[q], bx = J.q_epx[q], by = J.q_epy[q];
+            const double l0 = ay * 1.0 - 1.0 * by;
+            const double l1 = 1.0 * bx - ax * 1.0;
+            const double l2 = ax * by - ay * bx;
+            const double den = sqrt(l0 * l0 + l1 * l1);
+            uint4 q0, q1;
+            load_desc(J.qdesc + 32 * (size_t)q, q0, q1);
+            unsigned best = PLP_MAX_HAMMING_DIST, second = PLP_MAX_HAMMING_DIST;
+            int best_lvl = -1, second_lvl = -1, best_p = -1;
+            for (int p = 0; p < n; ++p) {
+                const float dsp = (float)((J.sx[p] * l0 + J.sy[p] * l1 + l2) / den);
+                const float dep = (float)((J.ex[p] * l0 + J.ey[p] * l1 + l2) / den);
+                if (fabsf(dsp) > margin || fabsf(dep) > margin) continue;
+                if (check_level) {
+                    const int oct = J.octave[p];
+                    if (oct < min_level) continue;
+                    if (max_level > 0 && oct > max_level) continue;
+                }
+                if (J.claimed && J.claimed[p]) continue;
+                if (owner[p] < q) continue;
+                if (rgbd_gate && J.xr_sp && J.xr_ep && J.q_xr_sp && J.q_xr_ep) {  // projection.cc:487-500
+                    if (J.xr_sp[p] > 0 && J.xr_ep[p] > 0) {
+                        const float e_sp = fabsf(J.q_xr_sp[q] - J.xr_sp[p]);
+                        const float e_ep = fabsf(J.q_xr_ep[q] - J.xr_ep[p]);
+                        if (margin < e_sp || margin < e_ep) continue;
                     }
                 }
-                if (best_p >= 0 && best <= (J.hamm_thr_p1 ? J.hamm_thr_p1 - 1u : (unsigned)PLP_HAMMING_DIST_THR_HIGH)) {
-                    bool ok = true;
-                    if (ratio_test && best_lvl == second_lvl && (float)best > lowe_ratio * (float)second) ok = false;
-                    if (ok) choice = best_p;
+                uint4 d0, d1;
+                load_desc(J.desc + 32 * (size_t)p, d0, d1);
+                const unsigned d = (unsigned)hamming256(q0, q1, d0, d1);
+                const int lvl = J.ratio_level ? J.ratio_level[p] : J.octave[p];
+                if (d < best) {
+                    second = best;
+                    best = d;
+                    second_lvl = best_lvl;
+                    best_lvl = lvl;
+                    best_p = p;
+                } else if (d < second) {
+                    second_lvl = lvl;
+                    second = d;
                 }
             }
-            J.choice[q] = choice;
-            if (choice >= 0) atomicMin(&owner_next[choice], q);
+            if (best_p >= 0 && best <= (J.hamm_thr_p1 ? J.hamm_thr_p1 - 1u : (unsigned)PLP_HAMMING_DIST_THR_HIGH)) {
+                bool ok = true;
+                if (ratio_test && best_lvl == second_lvl && (float)best > lowe_ratio * (float)second) ok = false;
+                if (ok) choice = best_p;
+            }
         }
-        __syncthreads();
-        for (int p = tid; p < n; p += kThreads)
-            if (owner_next[p] != owner_prev[p]) flags[0] = 1;
-        __syncthreads();
-        const int changed = flags[0];
-        __syncthreads();
-        if (!changed) break;
-        if (tid == 0) flags[0] = 0;
-        int *t = owner_prev;
-        owner_prev = owner_next;
-        owner_next = t;
-        for (int p = tid; p < n; p += kThreads) owner_next[p] = 0x7fffffff;
-        __syncthreads();
-    }
+        return choice;
+    });
     if (J.matched_out)
         for (int i = tid; i < n; i += kThreads) J.matched_out[i] = -1;
     __syncthreads();
@@ -335,76 +284,46 @@ __global__ void __launch_bounds__(kThreads, 1)
         load_desc(J.frm_desc + 32 * (size_t)i, d0, d1);
         sdesc[2 * i] = d0;
         sdesc[2 * i + 1] = d1;
-        owner_prev[i] = 0x7fffffff;
-        owner_next[i] = 0x7fffffff;
+        owner_prev[i] = kNoOwner;
+        owner_next[i] = kNoOwner;
     }
     if (tid < 4) flags[tid] = 0;
     for (int b = tid; b < kHistLen; b += kThreads) hist[b] = 0;
     __syncthreads();
-    for (int round = 0; round <= n2; ++round) {
-        for (int q = tid; q < n2; q += kThreads) {
-            int choice = -1;
-            const bool valid = J.kf_valid ? (J.kf_valid[q] != 0) : true;
-            if (valid) {
-                uint4 q0, q1;
-                load_desc(J.kf_desc + 32 * (size_t)q, q0, q1);
-                unsigned best = PLP_MAX_HAMMING_DIST, second = PLP_MAX_HAMMING_DIST;
-                int best_i = -1;
-                for (int i = 0; i < n1; ++i) {
-                    if (owner_prev[i] < q) continue;  // already_matched_indices_1
-                    const unsigned d = (unsigned)hamming256(q0, q1, sdesc[2 * i], sdesc[2 * i + 1]);
-                    if (d < best) {
-                        second = best;
-                        best = d;
-                        best_i = i;
-                    } else if (d < second) {
-                        second = d;
-                    }
+    claim_fixed_point(n2, n1, owner_prev, owner_next, &flags[0], J.choice, [&](int q, const int *owner) {
+        int choice = -1;
+        const bool valid = J.kf_valid ? (J.kf_valid[q] != 0) : true;
+        if (valid) {
+            uint4 q0, q1;
+            load_desc(J.kf_desc + 32 * (size_t)q, q0, q1);
+            unsigned best = PLP_MAX_HAMMING_DIST, second = PLP_MAX_HAMMING_DIST;
+            int best_i = -1;
+            for (int i = 0; i < n1; ++i) {
+                if (owner[i] < q) continue;  // already_matched_indices_1
+                const unsigned d = (unsigned)hamming256(q0, q1, sdesc[2 * i], sdesc[2 * i + 1]);
+                if (d < best) {
+                    second = best;
+                    best = d;
+                    best_i = i;
+                } else if (d < second) {
+                    second = d;
                 }
-                // robust.cc:335-349
-                if (!(PLP_HAMMING_DIST_THR_LOW < best) && best_i >= 0 && !(lowe_ratio * (float)second < (float)best))
-                    choice = best_i;
             }
-            J.choice[q] = choice;
-            if (choice >= 0) atomicMin(&owner_next[choice], q);
+            // robust.cc:335-349
+            if (!(PLP_HAMMING_DIST_THR_LOW < best) && best_i >= 0 && !(lowe_ratio * (float)second < (float)best))
+                choice = best_i;
         }
-        __syncthreads();
-        for (int i = tid; i < n1; i += kThreads)
-            if (owner_next[i] != owner_prev[i]) flags[0] = 1;
-        __syncthreads();
-        const int changed = flags[0];
-        __syncthreads();
-        if (!changed) break;
-        if (tid == 0) flags[0] = 0;
-        int *t = owner_prev;
-        owner_prev = owner_next;
-        owner_next = t;
-        for (int i = tid; i < n1; i += kThreads) owner_next[i] = 0x7fffffff;
-        __syncthreads();
-    }
+        return choice;
+    });
     for (int i = tid; i < n1; i += kThreads) J.matched_out[i] = -1;
     __syncthreads();
     const bool do_angle = check_orientation && J.frm_angle && J.kf_angle;
+    const auto delta = [&](int q, int i) { return J.frm_angle[i] - J.kf_angle[q]; };
+    orientation_check<kThreads>(n2, J.choice, do_angle, hist, bin_valid, &flags[1], delta);
     for (int q = tid; q < n2; q += kThreads) {
         const int i = J.choice[q];
         if (i < 0) continue;
-        atomicAdd(&flags[1], 1);
-        if (do_angle) atomicAdd(&hist[angle_bin(J.frm_angle[i] - J.kf_angle[q])], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-        if (do_angle)
-            rank_bins(hist, bin_valid);
-        else
-            for (int b = 0; b < kHistLen; ++b) bin_valid[b] = 1;
-    }
-    __syncthreads();
-    for (int q = tid; q < n2; q += kThreads) {
-        const int i = J.choice[q];
-        if (i < 0) continue;
-        bool keep = true;
-        if (do_angle) keep = bin_valid[angle_bin(J.frm_angle[i] - J.kf_angle[q])] != 0;
-        if (keep)
+        if (!do_angle || bin_valid[angle_bin(delta(q, i))])
             J.matched_out[i] = q;
         else
             atomicAdd(&flags[2], 1);
@@ -458,84 +377,53 @@ __global__ void __launch_bounds__(kThreads, 1) triangulation_match_kernel(const 
     int *flags = hist + kHistLen;
     uint8_t *bin_valid = reinterpret_cast<uint8_t *>(flags + 4);
     for (int j = tid; j < n2; j += kThreads) {
-        owner_prev[j] = 0x7fffffff;
-        owner_next[j] = 0x7fffffff;
+        owner_prev[j] = kNoOwner;
+        owner_next[j] = kNoOwner;
     }
     if (tid < 4) flags[tid] = 0;
     for (int b = tid; b < kHistLen; b += kThreads) hist[b] = 0;
     __syncthreads();
-    // Sequential semantics: step p takes the best candidate not taken by an earlier step.  Iterating
-    // "choice[p] = best candidate not owned by a step < p" reaches the unique fixed point (step p depends only on < p).
-    for (int round = 0; round <= P; ++round) {
-        for (int p = tid; p < P; p += kThreads) {
-            const int i1 = J.seq_idx1[p];
-            uint4 q0, q1;
-            load_desc(J.desc1 + 32 * (size_t)i1, q0, q1);
-            const double *b1 = J.bearing1 + 3 * (size_t)i1;
-            const bool st1 = J.stereo1 ? (J.stereo1[i1] != 0) : false;
-            const float sf1 = J.scale_factors1[J.octave1[i1]];
-            unsigned best = PLP_HAMMING_DIST_THR_LOW;
-            int best_j = -1;
-            for (int c = J.seq_cbeg[p]; c < J.seq_cend[p]; ++c) {
-                const int j = J.cand2[c];
-                if (J.has_lm2[j]) continue;
-                if (owner_prev[j] < p) continue;  // is_already_matched_in_keyfrm_2
-                uint4 d0, d1;
-                load_desc(J.desc2 + 32 * (size_t)j, d0, d1);
-                const unsigned d = (unsigned)hamming256(q0, q1, d0, d1);
-                if (PLP_HAMMING_DIST_THR_LOW < d || best < d) continue;
-                const double *b2 = J.bearing2 + 3 * (size_t)j;
-                const bool st2 = J.stereo2 ? (J.stereo2[j] != 0) : false;
-                if (!st1 && !st2) {
-                    const double cos_dist = J.epipole[0] * b2[0] + J.epipole[1] * b2[1] + J.epipole[2] * b2[2];
-                    if (0.99862953475 < cos_dist) continue;
-                }
-                if (check_epipolar_constraint(b1, b2, J.E, sf1)) {
-                    best_j = j;
-                    best = d;
-                }
+    // Sequential semantics: step p takes the best candidate not taken by an earlier step.
+    claim_fixed_point(P, n2, owner_prev, owner_next, &flags[0], J.choice, [&](int p, const int *owner) {
+        const int i1 = J.seq_idx1[p];
+        uint4 q0, q1;
+        load_desc(J.desc1 + 32 * (size_t)i1, q0, q1);
+        const double *b1 = J.bearing1 + 3 * (size_t)i1;
+        const bool st1 = J.stereo1 ? (J.stereo1[i1] != 0) : false;
+        const float sf1 = J.scale_factors1[J.octave1[i1]];
+        unsigned best = PLP_HAMMING_DIST_THR_LOW;
+        int best_j = -1;
+        for (int c = J.seq_cbeg[p]; c < J.seq_cend[p]; ++c) {
+            const int j = J.cand2[c];
+            if (J.has_lm2[j]) continue;
+            if (owner[j] < p) continue;  // is_already_matched_in_keyfrm_2
+            uint4 d0, d1;
+            load_desc(J.desc2 + 32 * (size_t)j, d0, d1);
+            const unsigned d = (unsigned)hamming256(q0, q1, d0, d1);
+            if (PLP_HAMMING_DIST_THR_LOW < d || best < d) continue;
+            const double *b2 = J.bearing2 + 3 * (size_t)j;
+            const bool st2 = J.stereo2 ? (J.stereo2[j] != 0) : false;
+            if (!st1 && !st2) {
+                const double cos_dist = J.epipole[0] * b2[0] + J.epipole[1] * b2[1] + J.epipole[2] * b2[2];
+                if (0.99862953475 < cos_dist) continue;
             }
-            J.choice[p] = best_j;
-            if (best_j >= 0) atomicMin(&owner_next[best_j], p);
+            if (check_epipolar_constraint(b1, b2, J.E, sf1)) {
+                best_j = j;
+                best = d;
+            }
         }
-        __syncthreads();
-        for (int j = tid; j < n2; j += kThreads)
-            if (owner_next[j] != owner_prev[j]) flags[0] = 1;
-        __syncthreads();
-        const int changed = flags[0];
-        __syncthreads();
-        if (!changed) break;
-        if (tid == 0) flags[0] = 0;
-        int *t = owner_prev;
-        owner_prev = owner_next;
-        owner_next = t;
-        for (int j = tid; j < n2; j += kThreads) owner_next[j] = 0x7fffffff;
-        __syncthreads();
-    }
+        return best_j;
+    });
     for (int i = tid; i < n1; i += kThreads) J.matched_out[i] = -1;
     __syncthreads();
     const bool do_angle = check_orientation && J.angle1 && J.angle2;
-    for (int p = tid; p < P; p += kThreads) {
-        const int j = J.choice[p];
-        if (j < 0) continue;
-        atomicAdd(&flags[1], 1);
-        if (do_angle) atomicAdd(&hist[angle_bin(J.angle1[J.seq_idx1[p]] - J.angle2[j])], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-        if (do_angle)
-            rank_bins(hist, bin_valid);
-        else
-            for (int b = 0; b < kHistLen; ++b) bin_valid[b] = 1;
-    }
-    __syncthreads();
+    const auto delta = [&](int p, int j) { return J.angle1[J.seq_idx1[p]] - J.angle2[j]; };
+    orientation_check<kThreads>(P, J.choice, do_angle, hist, bin_valid, &flags[1], delta);
     for (int p = tid; p < P; p += kThreads) {
         const int j = J.choice[p];
         if (j < 0) continue;
         const int i1 = J.seq_idx1[p];
-        bool keep = true;
-        if (do_angle) keep = bin_valid[angle_bin(J.angle1[i1] - J.angle2[j])] != 0;
-        if (keep)
+        if (!do_angle || bin_valid[angle_bin(delta(p, j))])
             J.matched_out[i1] = j;
         else
             atomicAdd(&flags[2], 1);

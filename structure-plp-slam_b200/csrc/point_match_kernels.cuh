@@ -5,10 +5,8 @@
 // for the host.
 //
 // One CTA (1024 threads) per frame.
-//   1-3  stable counting sort of the keypoints by (cell_x, cell_y, index) -- exactly the traversal order of
-//        get_keypoints_in_cell (data/common.cc:275-309): cell histogram (shared-memory atomics), block-wide exclusive scan,
-//        scatter with per-cell cursors (any order), then every cell is put back into index order by one thread (cells hold
-//        ~0.4 keypoints on average, 10 x 10 px) -- O(n), replaces the O(n^2) rank sort;
+//   1-3  stable counting sort of the keypoints by (cell_x, cell_y, index), sort_by_cell of match_common.cuh -- exactly
+//        the traversal order of get_keypoints_in_cell (data/common.cc:275-309);
 //   4    the reference's sequential greedy ("skip keypoints claimed by an earlier query") as a fixed point, see below;
 //        a GROUP of kGroup lanes owns one query: the lanes take the grid columns of the query window round-robin (a
 //        column's cells [min_cy, max_cy] are one contiguous span of the sorted arrays) and scan their spans
@@ -23,6 +21,7 @@
 
 #include "../../include/plpslam_b200.h"
 #include "devmath.cuh"
+#include "match_common.cuh"
 #include "match_jobs.h"
 
 namespace plp {
@@ -31,43 +30,7 @@ namespace pm {
 
 constexpr int kThreads = 1024;
 constexpr int kGroup = 4;        // lanes per query
-constexpr int kHistLen = 30;     // angle_checker.h:47
-constexpr int kNumBinsThr = 3;   // angle_checker.h:48
-constexpr int kNoOwner = 0x7fffffff;
 constexpr int kNoKey = 0x7fffffff;
-
-// angle_checker.h:100-113
-__device__ __forceinline__ int angle_bin(float delta_angle) {
-    if (delta_angle < 0.0) delta_angle = (float)((double)delta_angle + 360.0);
-    if (360.0 <= delta_angle) delta_angle = (float)((double)delta_angle - 360.0);
-    const float inv_len = 1.0f / (float)kHistLen;
-    return __float2int_rn(delta_angle * inv_len);
-}
-
-// angle_checker.h:163-175: rank bins by size (desc), ties by bin index (asc); first 3 are valid.  One thread.
-__device__ inline void rank_bins(const int *hist, uint8_t *bin_valid) {
-    bool used[kHistLen];
-    for (int b = 0; b < kHistLen; ++b) {
-        used[b] = false;
-        bin_valid[b] = 0;
-    }
-    for (int k = 0; k < kNumBinsThr; ++k) {
-        int best = -1, best_cnt = -1;
-        for (int b = 0; b < kHistLen; ++b)
-            if (!used[b] && hist[b] > best_cnt) {
-                best_cnt = hist[b];
-                best = b;
-            }
-        used[best] = true;
-        bin_valid[best] = 1;
-    }
-}
-
-__device__ __forceinline__ void load_desc(const uint8_t *p, uint4 &a, uint4 &b) {
-    const uint4 *q = reinterpret_cast<const uint4 *>(p);
-    a = __ldg(q);
-    b = __ldg(q + 1);
-}
 
 struct PointSmem {
     uint4 *desc;     // 2 per keypoint, sorted order
@@ -123,18 +86,6 @@ static inline size_t point_smem_bytes(int cap, int num_cols, int num_rows) {
            (size_t)(num_cols + 16);
 }
 
-// the window of query q in grid cells (data/common.cc:249-272); false if it misses the grid
-struct Window {
-    int min_cx, max_cx, min_cy, max_cy;
-};
-__device__ __forceinline__ bool query_window(const plp_grid &grid, float ref_x, float ref_y, float r, Window &w) {
-    w.min_cx = max(0, cv_floor((double)(ref_x - grid.min_x - r) * grid.inv_cell_width));
-    w.max_cx = min(grid.num_cols - 1, cv_ceil((double)(ref_x - grid.min_x + r) * grid.inv_cell_width));
-    w.min_cy = max(0, cv_floor((double)(ref_y - grid.min_y - r) * grid.inv_cell_height));
-    w.max_cy = min(grid.num_rows - 1, cv_ceil((double)(ref_y - grid.min_y + r) * grid.inv_cell_height));
-    return w.min_cx < grid.num_cols && w.max_cx >= 0 && w.min_cy < grid.num_rows && w.max_cy >= 0;
-}
-
 // Top-2 keys of query q over its window, computed by the kGroup lanes of a group (all lanes of the WARP must call it
 // together: the merge uses shuffles).  `active` = this group has a query to scan; `owner` (may be null): skip candidates
 // owned by a smaller query; `floor`: only keys strictly greater (-1 = none).
@@ -184,15 +135,7 @@ __device__ __forceinline__ void group_scan(const PointSmem &S, const PointMatchJ
             }
         }
     }
-#pragma unroll
-    for (int o = kGroup / 2; o > 0; o >>= 1) {
-        const int o1 = __shfl_xor_sync(0xffffffffu, k1, o);
-        const int o2 = __shfl_xor_sync(0xffffffffu, k2, o);
-        const int lo = k1 < o1 ? k1 : o1, hi = k1 < o1 ? o1 : k1;
-        const int s2 = k2 < o2 ? k2 : o2;
-        k1 = lo;
-        k2 = hi < s2 ? hi : s2;
-    }
+    warp_top2<kGroup>(k1, k2);
 }
 
 __device__ __forceinline__ bool group_any(bool v) {
@@ -209,7 +152,7 @@ __global__ void __launch_bounds__(kThreads, 1)
     const PointMatchJob &J = jobs[blockIdx.x];
     if (J.m < 0) return;  // job disabled (e.g. the widened-margin retry is not needed for this frame)
     PointSmem S = carve_point_smem(smem_raw, cap, grid.num_cols, grid.num_rows);
-    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, nwarps = kThreads / 32;
+    const int tid = threadIdx.x, lane = tid & 31;
     if (J.n > cap) {  // more keypoints than the shared-memory tables hold: report "no matches" loudly (0xffffffff)
         if (J.matched_out)
             for (int i = tid; i < J.n; i += kThreads) J.matched_out[i] = -1;
@@ -219,78 +162,11 @@ __global__ void __launch_bounds__(kThreads, 1)
         return;
     }
     const int n = J.n, m = J.m;
-    const int cells = grid.num_cols * grid.num_rows;
 
-    // ---- 1. cell key of every keypoint (data/common.h:104-109) and the cell histogram; owner_a doubles as key buffer
+    // ---- 1-3. stable sort by (cell key, index); owner_a doubles as key buffer
     int *key = S.owner_a;
-    for (int k = tid; k < cells + 2; k += kThreads) S.col_start[k] = 0;
     if (tid < 4) S.flags[tid] = 0;
-    __syncthreads();
-    for (int i = tid; i < n; i += kThreads) {
-        const float px = J.x[i], py = J.y[i];
-        const int cx = cv_floor((double)(px - grid.min_x) * grid.inv_cell_width);
-        const int cy = cv_floor((double)(py - grid.min_y) * grid.inv_cell_height);
-        const bool in = (0 <= cx && cx < grid.num_cols && 0 <= cy && cy < grid.num_rows);
-        const int k = in ? cx * grid.num_rows + cy : cells;  // out-of-grid keypoints sort last and are never visited
-        key[i] = k;
-        atomicAdd(&S.col_start[k], 1);
-    }
-    __syncthreads();
-    // ---- 2. exclusive scan of the histogram: col_start[k] = first sorted position whose cell key >= k
-    //         (k = cell_x * num_rows + cell_y), so the cells [min_cy, max_cy] of one grid column are ONE contiguous span
-    {
-        const int total = cells + 1;  // keys 0 .. cells
-        const int per = (total + kThreads - 1) / kThreads;
-        const int b0 = min(total, tid * per), b1 = min(total, b0 + per);
-        int sum = 0;
-        for (int k = b0; k < b1; ++k) sum += S.col_start[k];
-        int incl = sum;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-            const int v = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += v;
-        }
-        if (lane == 31) S.warp_sums[warp] = incl;
-        __syncthreads();
-        if (warp == 0) {
-            const int v = lane < nwarps ? S.warp_sums[lane] : 0;
-            int sc = v;
-#pragma unroll
-            for (int o = 1; o < 32; o <<= 1) {
-                const int u = __shfl_up_sync(0xffffffffu, sc, o);
-                if (lane >= o) sc += u;
-            }
-            if (lane < nwarps) S.warp_sums[lane] = sc - v;  // exclusive prefix of the warp totals
-        }
-        __syncthreads();
-        int run = S.warp_sums[warp] + incl - sum;
-        for (int k = b0; k < b1; ++k) {
-            const int v = S.col_start[k];
-            S.col_start[k] = run;
-            S.cursor[k] = run;
-            run += v;
-        }
-        if (tid == 0) S.col_start[cells + 1] = n;
-    }
-    __syncthreads();
-    // ---- 3. scatter (order inside a cell arbitrary), then restore index order inside every cell: together a stable
-    //         sort by (cell key, index) = the traversal order of get_keypoints_in_cell (data/common.cc:275-309)
-    for (int i = tid; i < n; i += kThreads) S.orig[atomicAdd(&S.cursor[key[i]], 1)] = i;
-    __syncthreads();
-    const int n_in = S.col_start[cells];
-    for (int k = tid; k < cells; k += kThreads) {
-        const int b0 = S.col_start[k], b1 = S.col_start[k + 1];
-        for (int a = b0 + 1; a < b1; ++a) {  // insertion sort of the (few) indices of one cell
-            const int v = S.orig[a];
-            int b = a - 1;
-            while (b >= b0 && S.orig[b] > v) {
-                S.orig[b + 1] = S.orig[b];
-                --b;
-            }
-            S.orig[b + 1] = v;
-        }
-    }
-    __syncthreads();
+    const int n_in = sort_by_cell<kThreads>(grid, n, J.x, J.y, key, S.col_start, S.cursor, S.warp_sums, S.orig);
     // gather the sorted keypoint data into shared memory
     for (int p = tid; p < n_in; p += kThreads) {
         const int i = S.orig[p];
@@ -408,11 +284,10 @@ __global__ void __launch_bounds__(kThreads, 1)
                 if (valid && round > 0) {
                     // a query's result depends only on the owners inside its column span: if none of them changed
                     // in the previous round the previous choice stands (it only re-issues its claim)
-                    const float ref_x = J.qx[q], r = J.qradius[q];
-                    const int min_cx = max(0, cv_floor((double)(ref_x - grid.min_x - r) * grid.inv_cell_width));
-                    const int max_cx = min(grid.num_cols - 1, cv_ceil((double)(ref_x - grid.min_x + r) * grid.inv_cell_width));
+                    Window w;
+                    query_window(grid, J.qx[q], J.qy[q], J.qradius[q], w);  // only the column range is used
                     bool dirty = false;
-                    for (int c = min_cx + gl; c <= max_cx; c += kGroup) dirty = dirty || S.colchg[c];
+                    for (int c = w.min_cx + gl; c <= w.max_cx; c += kGroup) dirty = dirty || S.colchg[c];
                     rescan = dirty;
                 }
                 if (round > 0) rescan = group_any(rescan);
@@ -474,28 +349,14 @@ __global__ void __launch_bounds__(kThreads, 1)
         for (int i = tid; i < n; i += kThreads) J.matched_out[i] = -1;
     __syncthreads();
     const bool do_angle = check_orientation && J.qangle != nullptr && J.angle != nullptr;
-    for (int q = tid; q < m; q += kThreads) {
-        const int p = J.choice[q];
-        if (p < 0) continue;
-        atomicAdd(&S.flags[1], 1);
-        if (do_angle) atomicAdd(&S.hist[angle_bin(J.qangle[q] - J.angle[S.orig[p]])], 1);
-    }
-    __syncthreads();
-    if (tid == 0) {
-        if (do_angle)
-            rank_bins(S.hist, S.bin_valid);
-        else
-            for (int b = 0; b < kHistLen; ++b) S.bin_valid[b] = 1;
-    }
-    __syncthreads();
+    const auto delta = [&](int q, int p) { return J.qangle[q] - J.angle[S.orig[p]]; };
+    orientation_check<kThreads>(m, J.choice, do_angle, S.hist, S.bin_valid, &S.flags[1], delta);
     for (int q = tid; q < m; q += kThreads) {
         const int p = J.choice[q];
         int out = -1;
         if (p >= 0) {
             const int i = S.orig[p];
-            bool keep = true;
-            if (do_angle) keep = S.bin_valid[angle_bin(J.qangle[q] - J.angle[i])] != 0;
-            if (keep) {
+            if (!do_angle || S.bin_valid[angle_bin(delta(q, p))]) {
                 out = i;
                 if (J.matched_out) J.matched_out[i] = q;
             } else {

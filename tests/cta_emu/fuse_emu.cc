@@ -1,5 +1,5 @@
 // fuse_emu.cc -- csrc/fuse_kernels.cuh (match::fuse search, GPU-verified) executed on the host: dynamic shared memory, the
-// stable counting sort with __match_any_sync, a 2-D grid (landmark chunks x targets).
+// stable counting sort with shared-memory atomics, a 2-D grid (landmark chunks x targets).
 #include "cta_emu.h"
 
 #include <string.h>

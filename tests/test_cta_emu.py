@@ -210,7 +210,7 @@ def test_bow_match_kernel_on_cpu_matches_oracle(bow_emu, orc, seed):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# match::fuse search kernel (GPU-verified, tests/test_fuse_gpu.py): dynamic shared memory, counting sort with __match_any
+# match::fuse search kernel (GPU-verified, tests/test_fuse_gpu.py): dynamic shared memory, counting sort with atomics
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def fuse_emu(tmp_path_factory):
