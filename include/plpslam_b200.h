@@ -761,6 +761,40 @@ PLP_API plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch,
                                                       int32_t *d_num_valid_out, int32_t *d_n_inliers_out,
                                                       int32_t *d_lm_iters_out);
 
+/* tracking_module::optimize_current_frame_with_local_map (tracking_module.cc:732-835), monocular points, for the frames
+ * of the tracker's most recent motion_track_batch_dev whose motion track succeeded (num_valid >= 20):
+ * search_local_landmarks (the landmarks the motion track matched are excluded, inliers and outliers of its pose
+ * optimisation alike; frame::can_observe at the motion-tracked pose; match_frame_and_landmarks with `margin` and Lowe
+ * ratio 0.8) -> pose_optimizer::optimize from the motion pose -> the outliers lose their landmark. */
+typedef struct plp_track_local { /* device pointers; frame b's local landmarks are rows [offsets[b], offsets[b+1]) in local_landmarks_ order */
+    const double *pos_w, *obs_mean_normal;                             /* x 3 */
+    const float *min_valid_dist, *max_valid_dist, *max_valid_dist_raw; /* get_min/max_valid_distance(), max_valid_dist_ */
+    const uint8_t *desc;                                               /* x 32 */
+    const uint8_t *valid;                                              /* !will_be_erased(); may be NULL */
+    const int32_t *offsets;                                            /* batch + 1 */
+    const int32_t *last_local_idx; /* one per plp_track_last row: that landmark's index in the same frame's local list, or -1 */
+} plp_track_local;
+
+/* Allocates the local-map scratch for max_batch frames of up to max_local_points local landmarks each and builds the
+ * predict_scale_level table for log_scale_factor (frame::log_scale_factor_, a float); call it once, outside the hot path. */
+PLP_API plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale_factor, int max_local_points);
+/* Follows motion_track_batch_dev for the same frames on the same stream (batch <= that call's batch), and reads its
+ * inputs and outputs: they must be intact.  No host synchronisation.  Outputs (device):
+ *   matched_out / local_out [batch x kp_capacity]: the last-frame row (as motion_track's matched_out) or the index in the
+ *     frame's local list that each keypoint holds after the outlier drop; the other entry is -1;
+ *   observable_out [rows of local]: can_observe passed (the caller's increase_num_observable);
+ *   pose_out [batch x 16]; num_tracked_out = inliers of the second pose optimisation (the caller applies 20, or 40
+ *     after relocalisation); n_inliers_out = the optimiser's return value; lm_iters_out;
+ *   status_out: 0, 1 = the frame's local list exceeds max_local_points, 2 = a last_local_idx entry is out of range.
+ * A frame whose motion track failed, or with status != 0, keeps the motion pose with every per-keypoint output -1, every
+ * observable flag 0, 0 iterations and num_tracked 0.  Without a reservation, or with batch > max_batch or no preceding
+ * motion track: PLP_ERR_INVALID and nothing is launched. */
+PLP_API plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, const plp_track_local *local,
+                                                         float margin, int32_t *d_matched_out, int32_t *d_local_out,
+                                                         uint8_t *d_observable_out, double *d_pose_out,
+                                                         int32_t *d_num_tracked_out, int32_t *d_n_inliers_out,
+                                                         int32_t *d_lm_iters_out, int32_t *d_status_out);
+
 /* ------------------------------------------------------------------------ */
 /* local bundle adjustment (optimize/local_bundle_adjuster*.cc)               */
 /* ------------------------------------------------------------------------ */

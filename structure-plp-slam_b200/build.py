@@ -36,6 +36,7 @@ FILE_FLAGS = {
     "essential.cu": NO_FMA,
     "plane.cu": NO_FMA,
     "camera.cu": NO_FMA,
+    "local_map.cu": NO_FMA,
 }
 
 

@@ -1,0 +1,187 @@
+// local_map.cu -- device-resident, frame-batched local-map tracking:
+//   tracking_module::optimize_current_frame_with_local_map (tracking_module.cc:732-835) =
+//       search_local_landmarks (frame::can_observe + projection::match_frame_and_landmarks, Lowe ratio 0.8)
+//     + pose_optimizer::optimize + the outlier drop and tracked-landmark count
+// for the batch of the tracker's most recent plp_tracker_motion_track_batch_dev, on the same stream and without leaving
+// HBM.  It reads that call's inputs, outputs and scratch (tracker.h) and writes separate outputs, so the motion
+// outputs stay as that call wrote them.  Device code: local_map_kernels.cuh.  The window matcher (ratio path) and the
+// pose optimiser are the existing launchers, and the predict_scale_level table is plp_fuse_level_thresholds'.
+//
+// This file is compiled with -fmad=false (build.py FILE_FLAGS): can_observe's double / float mix rounds like the oracle.
+#include "common.cuh"
+#include "local_map_kernels.cuh"
+#include "match_kernels.cuh"
+#include "pose_kernels.cuh"
+#include "tracker.h"
+
+namespace plp {
+
+namespace {
+
+using lm::LocalDev;
+using lm::local_finish_kernel;
+using lm::local_gather_kernel;
+using lm::local_observe_kernel;
+using lm::local_prep_kernel;
+
+// the scratch of plp_tracker_reserve_local_map, carved from one allocation (B frames, C keypoints, ML local rows)
+struct LocalLayout {
+    size_t excl, center, qx, qy, qr, qmin, qmax, qv, choice, best, nm, claimed, mjobs, posejobs, obs, obs_kp, obs_out;
+    size_t bytes;
+    LocalLayout(size_t B, size_t C, size_t ML) {
+        size_t off = 0;
+        auto take = [&](size_t n) {
+            const size_t o = off;
+            off += (n + 255) & ~(size_t)255;
+            return o;
+        };
+        excl = take(B * ML);
+        center = take(B * 3 * 8);
+        qx = take(B * ML * 4);
+        qy = take(B * ML * 4);
+        qr = take(B * ML * 4);
+        qmin = take(B * ML * 4);
+        qmax = take(B * ML * 4);
+        qv = take(B * ML);
+        choice = take(B * ML * 4);
+        best = take(B * ML * 4);
+        nm = take(B * 4);
+        claimed = take(B * C);
+        mjobs = take(B * sizeof(PointMatchJob));
+        posejobs = take(B * sizeof(PoseJob));
+        obs = take(B * C * sizeof(plp_pt_obs));
+        obs_kp = take(B * C * 4);
+        obs_out = take(B * C);
+        bytes = off;
+    }
+};
+
+}  // namespace
+
+}  // namespace plp
+
+using namespace plp;
+
+extern "C" {
+
+plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale_factor, int max_local_points) {
+    PLP_REQUIRE(t, "null pointer");
+    PLP_REQUIRE(max_local_points >= 1, "max_local_points");
+    float thr[16];
+    PLP_TRY(plp_fuse_level_thresholds(log_scale_factor, t->num_levels, thr));
+    PLP_CUDA_TRY(cudaSetDevice(t->ctx->device));
+    if (t->d_local) {  // a second reservation replaces the first once the stream has stopped using it
+        PLP_CUDA_TRY(cudaStreamSynchronize(t->ctx->stream));
+        cudaFree(t->d_local);
+        t->d_local = nullptr;
+        t->max_local = 0;
+    }
+    const LocalLayout lay(t->max_batch, t->cap, max_local_points);
+    if (cudaMalloc((void **)&t->d_local, lay.bytes) != cudaSuccess) {
+        t->d_local = nullptr;
+        set_error("tracker: cudaMalloc(%zu) for the local map failed", lay.bytes);
+        return PLP_ERR_CUDA;
+    }
+    t->max_local = max_local_points;
+    for (int k = 0; k < 16; ++k) t->level_thr[k] = k < t->num_levels ? thr[k] : INFINITY;
+    return PLP_OK;
+}
+
+plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, const plp_track_local *local, float margin,
+                                                 int32_t *d_matched_out, int32_t *d_local_out, uint8_t *d_observable_out,
+                                                 double *d_pose_out, int32_t *d_num_tracked_out, int32_t *d_n_inliers_out,
+                                                 int32_t *d_lm_iters_out, int32_t *d_status_out) {
+    PLP_REQUIRE(t && local && d_matched_out && d_local_out && d_observable_out && d_pose_out && d_num_tracked_out &&
+                    d_n_inliers_out && d_lm_iters_out && d_status_out,
+                "null pointer");
+    PLP_REQUIRE(local->pos_w && local->obs_mean_normal && local->min_valid_dist && local->max_valid_dist &&
+                    local->max_valid_dist_raw && local->desc && local->offsets && local->last_local_idx,
+                "local-map arrays");
+    PLP_REQUIRE(t->d_local, "plp_tracker_reserve_local_map has not been called");
+    PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
+    PLP_REQUIRE(t->has_motion && batch <= t->motion.batch,
+                "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
+    PLP_REQUIRE(margin > 0.0f, "margin");
+    plp_ctx *ctx = t->ctx;
+    PLP_CUDA_TRY(cudaSetDevice(ctx->device));
+    const TrackDev &M = t->motion;
+    const LocalLayout lay(t->max_batch, t->cap, t->max_local);
+    uint8_t *d = t->d_local;
+    LocalDev D;
+    memset(&D, 0, sizeof(D));
+    D.batch = batch;
+    D.cap = t->cap;
+    D.max_local = t->max_local;
+    D.n_kp = M.n_kp;
+    D.x = M.x;
+    D.y = M.y;
+    D.octave = M.octave;
+    D.desc = M.desc;
+    D.last_pos_w = M.last_pos_w;
+    D.last_offsets = M.last_offsets;
+    D.motion_matched = M.matched;
+    D.motion_pose = M.pose_out;
+    D.motion_num_valid = M.num_valid;
+    D.motion_jobs = M.posejobs;
+    D.obs_last = M.obs_last;
+    for (int l = 0; l < 16; ++l) D.inv_level_sigma_sq[l] = M.inv_level_sigma_sq[l];
+    D.pos_w = local->pos_w;
+    D.normal = local->obs_mean_normal;
+    D.min_d = local->min_valid_dist;
+    D.max_d = local->max_valid_dist;
+    D.max_raw = local->max_valid_dist_raw;
+    D.lm_desc = local->desc;
+    D.valid = local->valid;
+    D.offsets = local->offsets;
+    D.last_local_idx = local->last_local_idx;
+    D.cam = t->cam;
+    for (int l = 0; l < 16; ++l) {
+        D.scale_factors[l] = l < t->num_levels ? t->scale_factors[l] : 1.0f;
+        D.level_thr[l] = t->level_thr[l];
+    }
+    D.num_levels = t->num_levels;
+    D.margin = margin;
+    D.excl = d + lay.excl;
+    D.center = (double *)(d + lay.center);
+    D.qx = (float *)(d + lay.qx);
+    D.qy = (float *)(d + lay.qy);
+    D.qradius = (float *)(d + lay.qr);
+    D.qmin = (int32_t *)(d + lay.qmin);
+    D.qmax = (int32_t *)(d + lay.qmax);
+    D.qvalid = d + lay.qv;
+    D.choice = (int32_t *)(d + lay.choice);
+    D.best = (int32_t *)(d + lay.best);
+    D.num_matches = (uint32_t *)(d + lay.nm);
+    D.claimed = d + lay.claimed;
+    D.mjobs = (PointMatchJob *)(d + lay.mjobs);
+    D.posejobs = (PoseJob *)(d + lay.posejobs);
+    D.obs = (plp_pt_obs *)(d + lay.obs);
+    D.obs_kp = (int32_t *)(d + lay.obs_kp);
+    D.obs_outlier = d + lay.obs_out;
+    D.matched = d_matched_out;
+    D.local = d_local_out;
+    D.observable = d_observable_out;
+    D.pose = d_pose_out;
+    D.num_tracked = d_num_tracked_out;
+    D.n_inliers = d_n_inliers_out;
+    D.lm_iters = d_lm_iters_out;
+    D.status = d_status_out;
+
+    PLP_LAUNCH(ctx, local_prep_kernel, batch, lm::kThreads, 0, D);
+    PLP_CHECK_LAUNCH();
+    const dim3 ogrid(div_up(t->max_local, lm::kObserveThreads), batch);
+    PLP_LAUNCH(ctx, local_observe_kernel, ogrid, lm::kObserveThreads, 0, D);
+    PLP_CHECK_LAUNCH();
+    // projection::match_frame_and_landmarks: ratio test, no orientation check, claims resolved in local-list order
+    PLP_TRY(launch_point_match(ctx, D.mjobs, batch, t->cap > kMatchMaxPoints ? kMatchMaxPoints : t->cap, t->grid, 1,
+                               lm::kLoweRatio, 0));
+    PLP_LAUNCH(ctx, local_gather_kernel, batch, lm::kThreads, 0, D);
+    PLP_CHECK_LAUNCH();
+    plp_pose_opt_cfg cfg{4, 10};
+    PLP_TRY(launch_pose_opt(ctx, D.posejobs, batch, t->cap, t->cam, cfg));
+    PLP_LAUNCH(ctx, local_finish_kernel, batch, lm::kThreads, 0, D);
+    PLP_CHECK_LAUNCH();
+    return PLP_OK;
+}
+
+}  // extern "C"

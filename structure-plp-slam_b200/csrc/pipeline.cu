@@ -17,50 +17,13 @@
 #include "camera_kernels.cuh"
 #include "match_kernels.cuh"
 #include "pose_kernels.cuh"
+#include "tracker.h"
 
 namespace plp {
 
 namespace {
 
 constexpr int kNumMatchesThr = 20;  // frame_tracker::num_matches_thr_ (module/frame_tracker.h)
-
-struct TrackDev {
-    int batch, cap, num_levels;
-    // current frames (ORB output)
-    const plp_keypoint *kp;
-    const uint8_t *desc;
-    const int32_t *n_kp;
-    // last frames
-    const double *last_pos_w;
-    const int32_t *last_octave;
-    const float *last_angle;
-    const uint8_t *last_desc;
-    const uint8_t *last_valid;
-    const int32_t *last_offsets;
-    const double *pose_pred, *pose_last;
-    // scratch (SoA copies of the current keypoints, queries, jobs)
-    float *x, *y, *angle;
-    int32_t *octave;
-    float *qx, *qy, *qxr, *qradius;
-    int32_t *qmin, *qmax;
-    uint8_t *qvalid;
-    int32_t *choice;
-    uint32_t *num_matches;
-    ProjectJob *pjobs;       // 2 x batch (first attempt, retry)
-    PointMatchJob *mjobs;    // 2 x batch
-    PoseJob *posejobs;       // batch
-    plp_pt_obs *obs;         // batch x cap
-    int32_t *obs_kp;         // batch x cap : keypoint index of each observation
-    uint8_t *obs_outlier;    // batch x cap
-    float inv_level_sigma_sq[16];
-    // outputs
-    int32_t *matched;        // batch x cap : last-frame index per keypoint (-1: none) after discard_outliers
-    double *pose_out;        // batch x 16
-    int32_t *num_valid;      // batch
-    int32_t *n_inliers;      // batch (pose optimiser return value)
-    int32_t *lm_iters;       // batch
-    int max_last;
-};
 
 __global__ void track_prep_kernel(TrackDev T, float margin, int check_orientation) {
     const int b = blockIdx.x, tid = threadIdx.x;
@@ -169,6 +132,7 @@ __global__ void track_gather_kernel(TrackDev T) {
             o.inv_sigma_sq = T.inv_level_sigma_sq[T.octave[base + i]];
             T.obs[base + off] = o;
             T.obs_kp[base + off] = i;
+            T.obs_last[base + off] = q;
         }
         __syncthreads();
         if (tid == 0) {
@@ -232,22 +196,6 @@ bool distortion_is_identity(const plp_distortion *dist);
 plp_status launch_undistort(plp_ctx *ctx, const UndistJob &J);
 }  // namespace plp
 
-struct plp_tracker {
-    plp_ctx *ctx = nullptr;
-    int max_batch = 0, cap = 0, max_last = 0, num_levels = 0;
-    plp_camera cam;
-    plp_grid grid;
-    float scale_factors[16];
-    float inv_level_sigma_sq[16];
-    float *d_scale_factors = nullptr;
-    uint8_t *d_block = nullptr;  // one allocation carved into the scratch arrays
-    TrackDev dev;
-    bool distorted = false;
-    UndistJob undist;                  // camera and coefficients; kp / n_kp / batch set per call
-    plp_keypoint *d_undist = nullptr;  // max_batch x cap (inside d_block)
-    double *d_bearings = nullptr;      // max_batch x cap x 3
-};
-
 extern "C" {
 
 plp_status plp_tracker_create(plp_ctx *ctx, const plp_camera *cam, const plp_grid *grid, const float *scale_factors,
@@ -293,7 +241,7 @@ plp_status plp_tracker_create_ex(plp_ctx *ctx, const plp_camera *cam, const plp_
     const size_t o_qmin = take(B * M * 4), o_qmax = take(B * M * 4), o_qv = take(B * M), o_choice = take(B * M * 4);
     const size_t o_nm = take(B * 4), o_pj = take(2 * B * sizeof(ProjectJob)), o_mj = take(2 * B * sizeof(PointMatchJob));
     const size_t o_poj = take(B * sizeof(PoseJob)), o_obs = take(B * C * sizeof(plp_pt_obs)), o_okp = take(B * C * 4);
-    const size_t o_oout = take(B * C);
+    const size_t o_oout = take(B * C), o_olast = take(B * C * 4);
     const size_t o_ukp = distorted ? take(B * C * sizeof(plp_keypoint)) : 0, o_ub = distorted ? take(B * C * 24) : 0;
     if (cudaMalloc((void **)&t->d_block, off) != cudaSuccess) {
         set_error("tracker: cudaMalloc(%zu) failed", off);
@@ -327,6 +275,7 @@ plp_status plp_tracker_create_ex(plp_ctx *ctx, const plp_camera *cam, const plp_
     T.obs = (plp_pt_obs *)(d + o_obs);
     T.obs_kp = (int32_t *)(d + o_okp);
     T.obs_outlier = d + o_oout;
+    T.obs_last = (int32_t *)(d + o_olast);
     for (int l = 0; l < 16; ++l) T.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
     if (distorted) {
         t->distorted = true;
@@ -351,6 +300,7 @@ void plp_tracker_destroy(plp_tracker *t) {
     cudaSetDevice(t->ctx->device);
     cudaStreamSynchronize(t->ctx->stream);
     if (t->d_block) cudaFree(t->d_block);
+    if (t->d_local) cudaFree(t->d_local);
     delete t;
 }
 
@@ -366,6 +316,7 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
                     last->pose_last,
                 "last-frame arrays");
     plp_ctx *ctx = t->ctx;
+    t->has_motion = false;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     TrackDev T = t->dev;
     T.batch = batch;
@@ -414,6 +365,8 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
     PLP_TRY(launch_pose_opt(ctx, T.posejobs, batch, t->cap > 6144 ? 6144 : t->cap, t->cam, cfg));
     PLP_LAUNCH(ctx, track_finish_kernel, batch, 256, 0, T);
     PLP_CHECK_LAUNCH();
+    t->motion = T;
+    t->has_motion = true;
     return PLP_OK;
 }
 

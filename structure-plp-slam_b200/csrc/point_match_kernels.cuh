@@ -295,6 +295,10 @@ __global__ void __launch_bounds__(kThreads, 1)
                     if (gl == 0 && valid) {
                         const int choice = J.choice[q];
                         if (choice >= 0) atomicMin(&owner_next[choice], q);
+                    } else if (gl == 0 && q < m) {
+                        // a warp whose queries are all invalid skips the scan: choice[] is scratch and may hold an
+                        // earlier call's values, so an invalid query's "no match" is written here
+                        J.choice[q] = -1;
                     }
                     continue;
                 }

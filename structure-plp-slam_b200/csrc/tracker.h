@@ -1,0 +1,73 @@
+// tracker.h -- internal: the state of a plp_tracker, shared by pipeline.cu (motion_based_track) and local_map.cu
+// (optimize_current_frame_with_local_map, which reads what the motion call left on the device).
+#pragma once
+#include "common.cuh"
+#include "camera_jobs.h"
+#include "match_jobs.h"
+#include "pose_jobs.h"
+
+namespace plp {
+
+struct TrackDev {
+    int batch, cap, num_levels;
+    // current frames (ORB output)
+    const plp_keypoint *kp;
+    const uint8_t *desc;
+    const int32_t *n_kp;
+    // last frames
+    const double *last_pos_w;
+    const int32_t *last_octave;
+    const float *last_angle;
+    const uint8_t *last_desc;
+    const uint8_t *last_valid;
+    const int32_t *last_offsets;
+    const double *pose_pred, *pose_last;
+    // scratch (SoA copies of the current keypoints, queries, jobs)
+    float *x, *y, *angle;
+    int32_t *octave;
+    float *qx, *qy, *qxr, *qradius;
+    int32_t *qmin, *qmax;
+    uint8_t *qvalid;
+    int32_t *choice;
+    uint32_t *num_matches;
+    ProjectJob *pjobs;       // 2 x batch (first attempt, retry)
+    PointMatchJob *mjobs;    // 2 x batch
+    PoseJob *posejobs;       // batch
+    plp_pt_obs *obs;         // batch x cap
+    int32_t *obs_kp;         // batch x cap : keypoint index of each observation
+    int32_t *obs_last;       // batch x cap : last-frame row of each observation (before discard_outliers)
+    uint8_t *obs_outlier;    // batch x cap
+    float inv_level_sigma_sq[16];
+    // outputs
+    int32_t *matched;        // batch x cap : last-frame index per keypoint (-1: none) after discard_outliers
+    double *pose_out;        // batch x 16
+    int32_t *num_valid;      // batch
+    int32_t *n_inliers;      // batch (pose optimiser return value)
+    int32_t *lm_iters;       // batch
+    int max_last;
+};
+
+}  // namespace plp
+
+struct plp_tracker {
+    plp_ctx *ctx = nullptr;
+    int max_batch = 0, cap = 0, max_last = 0, num_levels = 0;
+    plp_camera cam;
+    plp_grid grid;
+    float scale_factors[16];
+    float inv_level_sigma_sq[16];
+    float *d_scale_factors = nullptr;
+    uint8_t *d_block = nullptr;  // one allocation carved into the scratch arrays
+    plp::TrackDev dev;
+    bool distorted = false;
+    plp::UndistJob undist;             // camera and coefficients; kp / n_kp / batch set per call
+    plp_keypoint *d_undist = nullptr;  // max_batch x cap (inside d_block)
+    double *d_bearings = nullptr;      // max_batch x cap x 3
+    // the most recent motion_track_batch_dev: its inputs, outputs and scratch, which local_map_track_batch_dev reads
+    plp::TrackDev motion;
+    bool has_motion = false;
+    // local-map tracking (plp_tracker_reserve_local_map); d_local == nullptr until reserved
+    int max_local = 0;
+    float level_thr[16];             // predict_scale_level thresholds (plp_fuse_level_thresholds)
+    uint8_t *d_local = nullptr;      // one allocation, carved by local_map.cu
+};

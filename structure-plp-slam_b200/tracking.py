@@ -1,7 +1,8 @@
-"""Device-resident batched front-end: ORB extraction + motion-based tracking without leaving HBM.
+"""Device-resident batched front-end: ORB extraction + motion-based tracking (+ optionally the local-map stage) without
+leaving HBM.
 
-Thin ctypes layer over plp_orb_extract_batch_dev + plp_tracker_motion_track_batch_dev; used by bench.py and
-the pipeline parity tests.  No compute here.
+Thin ctypes layer over plp_orb_extract_batch_dev + plp_tracker_motion_track_batch_dev (+
+plp_tracker_local_map_track_batch_dev); used by bench.py and the pipeline parity tests.  No compute here.
 """
 from __future__ import annotations
 
@@ -16,6 +17,19 @@ from .capi import (KP_DTYPE, Context, OrbExtractor, PlpError, _P, make_camera, m
 class TrackLast(C.Structure):
     _fields_ = [("pos_w", _P), ("octave", _P), ("angle", _P), ("desc", _P), ("valid", _P), ("offsets", _P),
                 ("pose_pred", _P), ("pose_last", _P)]
+
+
+class TrackLocal(C.Structure):
+    _fields_ = [("pos_w", _P), ("obs_mean_normal", _P), ("min_valid_dist", _P), ("max_valid_dist", _P),
+                ("max_valid_dist_raw", _P), ("desc", _P), ("valid", _P), ("offsets", _P), ("last_local_idx", _P)]
+
+
+def _logf(x: float) -> float:
+    """The C library's logf: frame::log_scale_factor_ = std::log(scale_factor_) on a float."""
+    libm = C.CDLL("libm.so.6")
+    libm.logf.restype = C.c_float
+    libm.logf.argtypes = [C.c_float]
+    return float(libm.logf(float(np.float32(x))))
 
 
 class DeviceBuffer:
@@ -134,6 +148,10 @@ class FrontEnd:
         self.d_num_valid = DeviceBuffer(ctx, B * 4)
         self.d_n_inl = DeviceBuffer(ctx, B * 4)
         self.d_lm = DeviceBuffer(ctx, B * 4)
+        self.scale_factor = scale_factor
+        self._local_bufs = []
+        self._local = None
+        self._local_out = None
         self._last_bufs = []
         self._last = None
         self._last_pinned = []   # host copies of the last-frame arrays (end-to-end path: uploaded every step)
@@ -142,6 +160,9 @@ class FrontEnd:
         self._out_layout = None
 
     def close(self):
+        for b in self._local_bufs:
+            b.free()
+        self._local_bufs = []
         if self._trk is not None:
             self.lib.plp_tracker_destroy(self._trk)
             self._trk = None
@@ -169,6 +190,44 @@ class FrontEnd:
         for b in self._last_pinned:
             b.free()
         self._last_pinned = [PinnedBuffer.from_array(self.ctx, a) for a in arrays]
+
+    def reserve_local_map(self, max_local_points: int):
+        """Scratch for local maps of up to max_local_points landmarks per frame (outside the hot path), and the
+        outputs of track_local_map."""
+        self.ctx._check(self.lib.plp_tracker_reserve_local_map(self._trk, C.c_float(_logf(self.scale_factor)),
+                                                           C.c_int(max_local_points)))
+        self.max_local = int(max_local_points)
+        B = self.max_batch
+        if self._local_out is None:
+            self._local_out = dict(matched=DeviceBuffer(self.ctx, B * self.cap * 4),
+                                   local=DeviceBuffer(self.ctx, B * self.cap * 4), pose=DeviceBuffer(self.ctx, B * 128),
+                                   num_tracked=DeviceBuffer(self.ctx, B * 4), n_inliers=DeviceBuffer(self.ctx, B * 4),
+                                   lm_iters=DeviceBuffer(self.ctx, B * 4), status=DeviceBuffer(self.ctx, B * 4))
+
+    def set_local_maps(self, local_list):
+        """local_list[b]: dict(pos_w[m,3], normal[m,3] (get_obs_mean_normal), min_valid_dist[m], max_valid_dist[m]
+        (get_min/max_valid_distance), max_valid_dist_raw[m] (max_valid_dist_), desc[m,32], valid[m]|None
+        (!will_be_erased), last_local_idx[rows of frame b in set_last_frames] (-1: not in the local list)), in
+        local_landmarks_ order."""
+        for b in self._local_bufs:
+            b.free()
+        offs = np.zeros(len(local_list) + 1, np.int32)
+        offs[1:] = np.cumsum([len(l["max_valid_dist"]) for l in local_list])
+
+        def cat(k, dt, shape):
+            parts = [np.asarray(l[k], dt).reshape((-1,) + shape) for l in local_list]
+            return np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0,) + shape, dt))
+        valid = np.ascontiguousarray(np.concatenate(
+            [np.asarray(l["valid"], np.uint8) if l.get("valid") is not None else np.ones(len(l["max_valid_dist"]), np.uint8)
+             for l in local_list]))
+        arrays = [cat("pos_w", np.float64, (3,)), cat("normal", np.float64, (3,)), cat("min_valid_dist", np.float32, ()),
+                  cat("max_valid_dist", np.float32, ()), cat("max_valid_dist_raw", np.float32, ()),
+                  cat("desc", np.uint8, (32,)), valid, offs, cat("last_local_idx", np.int32, ())]
+        self._local_bufs = [DeviceBuffer.from_array(self.ctx, a) for a in arrays]
+        self._local = TrackLocal(*[b.ptr for b in self._local_bufs])
+        self._local_offsets = offs
+        self._d_observable = DeviceBuffer(self.ctx, max(int(offs[-1]), 1))
+        self._local_bufs.append(self._d_observable)
 
     # -- end-to-end path: every input of a step comes from pinned host memory, every result goes back ----
     def stage_host_io(self, imgs: np.ndarray):
@@ -249,6 +308,17 @@ class FrontEnd:
         self.extract(batch)
         self.track(batch, margin)
 
+    def track_local_map(self, batch: int, margin: float = 5.0):
+        """optimize_current_frame_with_local_map for the batch of the preceding track() (tracking stream).  margin:
+        5, or 20 for a recently relocalised frame (tracking_module.cc:976-981)."""
+        o = self._local_out
+        if o is None or self._local is None:
+            raise PlpError("track_local_map needs reserve_local_map() and set_local_maps() first")
+        self.ctx._check(self.lib.plp_tracker_local_map_track_batch_dev(
+            self._trk, C.c_int(batch), C.byref(self._local), C.c_float(margin), o["matched"].ptr, o["local"].ptr,
+            self._d_observable.ptr, o["pose"].ptr, o["num_tracked"].ptr, o["n_inliers"].ptr, o["lm_iters"].ptr,
+            o["status"].ptr))
+
     # -- results --------------------------------------------------------------------------------------
     def _after_tracking(self):
         """The downloads below run on the extraction stream; the tracking outputs are written on the tracking stream."""
@@ -277,6 +347,25 @@ class FrontEnd:
         self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, kp.ctypes.data_as(_P), kp_p, C.c_size_t(kp.nbytes)))
         self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, bear.ctypes.data_as(_P), b_p, C.c_size_t(bear.nbytes)))
         return [(kp[b, :n[b]].copy(), bear[b, :n[b]].copy()) for b in range(batch)]
+
+    def download_local_tracking(self, batch: int):
+        """Results of track_local_map: per frame the last-frame row / local-list index held by each keypoint, the
+        observable flag of every local row, pose, num_tracked, n_inliers, LM iterations and status."""
+        self._after_tracking()
+        n = self.d_n.download(np.int32, (batch,))
+        o = self._local_out
+        matched = o["matched"].download(np.int32, (self.max_batch, self.cap))[:batch]
+        local = o["local"].download(np.int32, (self.max_batch, self.cap))[:batch]
+        offs = self._local_offsets
+        obs = self._d_observable.download(np.uint8, (max(int(offs[-1]), 1),))
+        return dict(matched=[matched[b, :n[b]].copy() for b in range(batch)],
+                    local=[local[b, :n[b]].copy() for b in range(batch)],
+                    observable=[obs[offs[b]:offs[b + 1]].copy() for b in range(batch)],
+                    pose=o["pose"].download(np.float64, (batch, 4, 4)),
+                    num_tracked=o["num_tracked"].download(np.int32, (batch,)),
+                    n_inliers=o["n_inliers"].download(np.int32, (batch,)),
+                    lm_iters=o["lm_iters"].download(np.int32, (batch,)),
+                    status=o["status"].download(np.int32, (batch,)))
 
     def download_tracking(self, batch: int):
         self._after_tracking()
