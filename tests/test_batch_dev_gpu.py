@@ -255,7 +255,8 @@ def test_line_batch_dev_automatic_kernel_choice(ctx, orc, plp):
     """plp_line_extract_batch_dev with caller buffers, an odd pitch and a caller status array, at batches where the
     automatic mode picks each region-growing kernel in turn: the multi-warp kernel for at most half a wave of frames,
     the shared-memory image kernel up to half of what stays resident (two frames per SM at 640 x 480), the L2 image
-    kernel above (the benchmark's 12 frames per SM)."""
+    kernel above (the benchmark's 12 frames per SM).  A live frame through the host entry point takes the out-of-order
+    kernel, the fastest for one frame."""
     from plpslam_b200.tracking import DeviceBuffer
     lib = plp.lib()
     sm = _sm_count(ctx.device)
@@ -287,6 +288,10 @@ def test_line_batch_dev_automatic_kernel_choice(ctx, orc, plp):
             _compare_lines(trk, orc, frames[b], b=b, got=(kl[b, :n[b]], lbd[b, :n[b]], fn[b, :n[b]]))
         assert n.min() > 40
         d_st.free()
+    live = []
+    names = _kernels_run(ctx, lib, lambda: live.append(trk.extract_LSD_LBD(frames[0])))
+    assert names & grow == {"lsd_grow_ooo_kernel"}, names
+    _compare_lines(trk, orc, frames[0], got=live[0])
     for d in (d_img, d_kl, d_lbd, d_fn, d_n):
         d.free()
     trk.close()

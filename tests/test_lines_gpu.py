@@ -4,14 +4,11 @@ functions.  Bar: bit-exact (the oracle's "det" mode is itself pinned bit-exactly
 import numpy as np
 import pytest
 
-import os
-
 import oracle_api
 import synth
 
 pytestmark = pytest.mark.gpu
-# all three region-growing variants; PLP_TEST_OOO=0 leaves the out-of-order one (3) out
-VARIANTS = [1, 2] if os.environ.get("PLP_TEST_OOO") == "0" else [1, 2, 3]
+VARIANTS = [1, 2, 3]
 
 KL_FIELDS = ("angle", "class_id", "octave", "pt_x", "pt_y", "response", "size", "start_x", "start_y", "end_x", "end_y",
              "s_oct_x", "s_oct_y", "e_oct_x", "e_oct_y", "line_length", "num_pixels")

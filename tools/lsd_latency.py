@@ -3,7 +3,6 @@
 python tools/lsd_latency.py"""
 import ctypes as C
 import json
-import os
 import sys
 import time
 from pathlib import Path
@@ -50,7 +49,7 @@ for kind, fr in frames.items():
         imgs = np.concatenate([fr] * ((batch + 7) // 8))[:batch]
         trk = plp.LineFeatureTracker(ctx, H, W, max_batch=batch)
         out = {}
-        for variant in ((1, 2) if os.environ.get('PLP_TEST_OOO') == '0' else (1, 2, 3)):
+        for variant in (1, 2, 3):
             trk.grow_variant(variant)
             out[variant] = (timed(trk, imgs), kernel_ms(trk, imgs))
             if variant == 2:
@@ -59,7 +58,7 @@ for kind, fr in frames.items():
         n = len(trk.extract_batch(imgs)[0][0])
         print(f"{kind:8s} batch={batch:3d} keylines[0]={n:4d}  one-warp: {out[1][0]:7.2f} ms/call (grow {out[1][1].get('lsd_grow')})"
               f"   multi-warp: {out[2][0]:7.2f} ms/call (grow {out[2][1].get('lsd_grow_mw')})  stats {st}\n"
-              + (f"          out-of-order: {out[3][0]:7.2f} ms/call (grow {out[3][1].get('lsd_grow_ooo')})  stats {st3}" if 3 in out else ""))
+              f"          out-of-order: {out[3][0]:7.2f} ms/call (grow {out[3][1].get('lsd_grow_ooo')})  stats {st3}")
         if batch == 1 and kind == "plp":
             print("    kernels (multi-warp run):", out[2][1])
         trk.close()
