@@ -11,7 +11,6 @@
 // one warp per shared node, sequential over the node's side-1 keypoints, lanes over its side-2 candidates (top-2 by
 // (distance, list position)), one CTA per (side-1, side-2) pair so that the orientation histogram is a block reduction.
 #include "common.cuh"
-#include "pack.cuh"
 #include "bow_kernels.cuh"
 
 #include <algorithm>
@@ -223,16 +222,19 @@ plp_status plp_bow_transform(plp_bow_vocab *v, const uint8_t *desc, int n, int l
     PLP_REQUIRE(desc && word_id_out && node_id_out && weight_out, "null pointer");
     plp_ctx *ctx = v->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    Packer pk;
-    const size_t o_d = pk.add(desc, (size_t)n * 32);
-    const size_t o_w = pk.reserve((size_t)n * 4), o_n = pk.reserve((size_t)n * 4), o_f = pk.reserve((size_t)n * 4);
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    PLP_TRY(launch_transform(v, d + o_d, n, levelsup, Packer::at<int32_t>(d, o_w), Packer::at<int32_t>(d, o_n),
-                             Packer::at<float>(d, o_f)));
-    PLP_CUDA_TRY(cudaMemcpyAsync(word_id_out, d + o_w, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(node_id_out, d + o_n, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(weight_out, d + o_f, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    DevLayout L;
+    const uint8_t *d_desc;
+    int32_t *d_word, *d_node;
+    float *d_weight;
+    L.in(d_desc, desc, (size_t)n * 32);
+    L.out(d_word, n);
+    L.out(d_node, n);
+    L.out(d_weight, n);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_transform(v, d_desc, n, levelsup, d_word, d_node, d_weight));
+    PLP_CUDA_TRY(to_host(ctx, word_id_out, d_word, n));
+    PLP_CUDA_TRY(to_host(ctx, node_id_out, d_node, n));
+    PLP_CUDA_TRY(to_host(ctx, weight_out, d_weight, n));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return PLP_OK;
 }
@@ -241,12 +243,14 @@ plp_status plp_match_bow_tree(plp_ctx *ctx, plp_bow_pair *pairs, int num_pairs, 
     PLP_REQUIRE(ctx && num_pairs >= 0, "ctx / num_pairs");
     if (num_pairs == 0) return PLP_OK;
     PLP_REQUIRE(pairs, "pairs");
-    struct SideOff {
-        size_t desc, angle, valid, idx;
+    struct SideDev {
+        const uint8_t *desc, *valid;
+        const float *angle;
+        const uint32_t *idx;
         std::vector<uint32_t> flat;  // validated copy of fv.indices
     };
-    std::map<const plp_bow_side *, SideOff> sides;
-    Packer pk;
+    std::map<const plp_bow_side *, SideDev> sides;  // node-based: the fields stay put once declared
+    DevLayout L;
     // validate + pack every distinct side once
     for (int p = 0; p < num_pairs; ++p) {
         pairs[p].num_matches = 0;
@@ -257,7 +261,7 @@ plp_status plp_match_bow_tree(plp_ctx *ctx, plp_bow_pair *pairs, int num_pairs, 
             PLP_REQUIRE(s->n == 0 || s->desc, "side descriptors");
             PLP_REQUIRE(s->fv.num_nodes == 0 || (s->fv.node_ids && s->fv.offsets && s->fv.indices), "feature vector");
             PLP_REQUIRE(!check_orientation || s->n == 0 || s->angle, "angles required for the orientation check");
-            SideOff so;
+            SideDev so;
             const int total = s->fv.num_nodes ? s->fv.offsets[s->fv.num_nodes] : 0;
             std::vector<uint8_t> seen((size_t)s->n, 0);
             for (int a = 0; a < s->fv.num_nodes; ++a) {
@@ -275,19 +279,19 @@ plp_status plp_match_bow_tree(plp_ctx *ctx, plp_bow_pair *pairs, int num_pairs, 
     }
     for (auto &kv : sides) {
         const plp_bow_side *s = kv.first;
-        SideOff &so = kv.second;
+        SideDev &so = kv.second;
         const size_t n = (size_t)s->n;
-        so.desc = pk.add(n ? s->desc : nullptr, n * 32);
-        so.angle = pk.add(n ? s->angle : nullptr, n * 4);
-        so.valid = pk.add(n ? s->valid : nullptr, n);
-        so.idx = pk.add(so.flat.empty() ? nullptr : so.flat.data(), so.flat.size() * 4);
+        L.in(so.desc, n ? s->desc : nullptr, n * 32);
+        L.in(so.angle, n ? s->angle : nullptr, n);
+        L.in(so.valid, n ? s->valid : nullptr, n);
+        L.in(so.idx, so.flat.empty() ? nullptr : so.flat.data(), so.flat.size());
     }
+    std::vector<BowJob> jobs(num_pairs);
     // merge-join of the two ascending feature vectors per pair (bow_tree.cc:60-150): the shared nodes
-    struct PairOff {
+    struct SharedNodes {
         std::vector<int32_t> nb1, ne1, nb2, ne2;
-        size_t o_nb1, o_ne1, o_nb2, o_ne2, o_claimed, o_choice, o_m21, o_m12, o_num;
     };
-    std::vector<PairOff> po(num_pairs);
+    std::vector<SharedNodes> po(num_pairs);
     for (int p = 0; p < num_pairs; ++p) {
         const plp_bow_feature_vector &f1 = pairs[p].side1->fv, &f2 = pairs[p].side2->fv;
         int a = 0, b = 0;
@@ -306,73 +310,49 @@ plp_status plp_match_bow_tree(plp_ctx *ctx, plp_bow_pair *pairs, int num_pairs, 
             }
         }
         const size_t nn = po[p].nb1.size(), n1 = (size_t)pairs[p].side1->n, n2 = (size_t)pairs[p].side2->n;
-        po[p].o_nb1 = pk.add(nn ? po[p].nb1.data() : nullptr, nn * 4);
-        po[p].o_ne1 = pk.add(nn ? po[p].ne1.data() : nullptr, nn * 4);
-        po[p].o_nb2 = pk.add(nn ? po[p].nb2.data() : nullptr, nn * 4);
-        po[p].o_ne2 = pk.add(nn ? po[p].ne2.data() : nullptr, nn * 4);
-        po[p].o_claimed = pk.reserve(n2 + 1);
-        po[p].o_choice = pk.reserve(n1 * 4 + 4);
-    }
-    // all results in ONE contiguous region -> one D2H copy (a copy per pair and array costs more than the kernel)
-    const size_t o_out0 = pk.total;
-    for (int p = 0; p < num_pairs; ++p) {
-        const size_t n1 = (size_t)pairs[p].side1->n, n2 = (size_t)pairs[p].side2->n;
-        po[p].o_m21 = pk.reserve(n1 * 4 + 4);
-        po[p].o_m12 = pk.reserve(n2 * 4 + 4);
-        po[p].o_num = pk.reserve(4);
-    }
-    const size_t o_out1 = pk.total;
-    std::vector<BowJob> jobs(num_pairs);
-    const size_t o_jobs = pk.add(jobs.data(), sizeof(BowJob) * (size_t)num_pairs);
-    PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    void *dscratch = nullptr;
-    PLP_TRY(ctx_scratch(ctx, 0, pk.total ? pk.total : 256, &dscratch));
-    uint8_t *d = (uint8_t *)dscratch;
-    for (int p = 0; p < num_pairs; ++p) {
         BowJob &J = jobs[p];
         memset(&J, 0, sizeof(J));
-        const SideOff &s1 = sides[pairs[p].side1], &s2 = sides[pairs[p].side2];
-        J.n1 = pairs[p].side1->n;
-        J.n2 = pairs[p].side2->n;
-        J.num_nodes = (int)po[p].nb1.size();
-        J.desc1 = Packer::at<uint8_t>(d, s1.desc);
-        J.desc2 = Packer::at<uint8_t>(d, s2.desc);
-        J.angle1 = Packer::at<float>(d, s1.angle);
-        J.angle2 = Packer::at<float>(d, s2.angle);
-        J.valid1 = Packer::at<uint8_t>(d, s1.valid);
-        J.valid2 = Packer::at<uint8_t>(d, s2.valid);
-        J.idx1 = Packer::at<uint32_t>(d, s1.idx);
-        J.idx2 = Packer::at<uint32_t>(d, s2.idx);
-        J.nb1 = Packer::at<int32_t>(d, po[p].o_nb1);
-        J.ne1 = Packer::at<int32_t>(d, po[p].o_ne1);
-        J.nb2 = Packer::at<int32_t>(d, po[p].o_nb2);
-        J.ne2 = Packer::at<int32_t>(d, po[p].o_ne2);
-        J.claimed = Packer::at<uint8_t>(d, po[p].o_claimed);
-        J.choice = Packer::at<int32_t>(d, po[p].o_choice);
-        J.matched_2_of_1 = Packer::at<int32_t>(d, po[p].o_m21);
-        J.matched_1_of_2 = Packer::at<int32_t>(d, po[p].o_m12);
-        J.num_matches = Packer::at<uint32_t>(d, po[p].o_num);
+        const SideDev &s1 = sides[pairs[p].side1], &s2 = sides[pairs[p].side2];
+        J.n1 = (int)n1;
+        J.n2 = (int)n2;
+        J.num_nodes = (int)nn;
+        L.same(J.desc1, s1.desc);
+        L.same(J.desc2, s2.desc);
+        L.same(J.angle1, s1.angle);
+        L.same(J.angle2, s2.angle);
+        L.same(J.valid1, s1.valid);
+        L.same(J.valid2, s2.valid);
+        L.same(J.idx1, s1.idx);
+        L.same(J.idx2, s2.idx);
+        L.in(J.nb1, nn ? po[p].nb1.data() : nullptr, nn);
+        L.in(J.ne1, nn ? po[p].ne1.data() : nullptr, nn);
+        L.in(J.nb2, nn ? po[p].nb2.data() : nullptr, nn);
+        L.in(J.ne2, nn ? po[p].ne2.data() : nullptr, nn);
+        L.out(J.claimed, n2 + 1);
+        L.out(J.choice, n1 + 1);
     }
-    uint8_t *d2;
-    PLP_TRY(pk.upload(ctx, 0, &d2));
-    if (d2 != d) {
-        set_error("bow_tree: scratch buffer moved between sizing and upload");
-        return PLP_ERR_CUDA;
+    // all results in ONE contiguous region -> one D2H copy (a copy per pair and array costs more than the kernel)
+    for (int p = 0; p < num_pairs; ++p) {
+        L.out(jobs[p].matched_2_of_1, (size_t)pairs[p].side1->n + 1);
+        L.out(jobs[p].matched_1_of_2, (size_t)pairs[p].side2->n + 1);
+        L.out(jobs[p].num_matches, 1);
     }
-    PLP_LAUNCH(ctx, bow_match_kernel, num_pairs, kMatchThreads, 0, Packer::at<BowJob>(d, o_jobs), lowe_ratio,
-               check_orientation);
+    const BowJob *d_jobs;
+    L.in(d_jobs, jobs.data(), num_pairs);
+    PLP_CUDA_TRY(cudaSetDevice(ctx->device));
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_LAUNCH(ctx, bow_match_kernel, num_pairs, kMatchThreads, 0, d_jobs, lowe_ratio, check_orientation);
     PLP_CHECK_LAUNCH();
-    void *hp = nullptr;
-    PLP_TRY(ctx_pinned(ctx, pk.total ? pk.total : 256, &hp));  // the staging buffer upload() just used
-    uint8_t *h = (uint8_t *)hp;
-    PLP_CUDA_TRY(cudaMemcpyAsync(h + o_out0, d + o_out0, o_out1 - o_out0, cudaMemcpyDeviceToHost, ctx->stream));
+    const uint8_t *out0 = (const uint8_t *)jobs.front().matched_2_of_1;
+    const uint8_t *out1 = (const uint8_t *)(jobs.back().num_matches + 1);
+    PLP_CUDA_TRY(cudaMemcpyAsync(L.host(out0), out0, out1 - out0, cudaMemcpyDeviceToHost, ctx->stream));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     std::vector<uint32_t> nums(num_pairs, 0);
     for (int p = 0; p < num_pairs; ++p) {
-        const size_t n1 = (size_t)pairs[p].side1->n, n2 = (size_t)pairs[p].side2->n;
-        if (pairs[p].matched_2_of_1_out && n1) memcpy(pairs[p].matched_2_of_1_out, h + po[p].o_m21, n1 * 4);
-        if (pairs[p].matched_1_of_2_out && n2) memcpy(pairs[p].matched_1_of_2_out, h + po[p].o_m12, n2 * 4);
-        memcpy(&nums[p], h + po[p].o_num, 4);
+        const BowJob &J = jobs[p];
+        if (pairs[p].matched_2_of_1_out && J.n1) memcpy(pairs[p].matched_2_of_1_out, L.host(J.matched_2_of_1), J.n1 * 4);
+        if (pairs[p].matched_1_of_2_out && J.n2) memcpy(pairs[p].matched_1_of_2_out, L.host(J.matched_1_of_2), J.n2 * 4);
+        nums[p] = *L.host(J.num_matches);
     }
     for (int p = 0; p < num_pairs; ++p) pairs[p].num_matches = nums[p];
     return PLP_OK;

@@ -9,7 +9,6 @@
 // (rectmath.h), converted to cv::remap's fixed point and kept on the device; rectify_kernel (rectify_kernels.cuh) remaps a
 // batch of one side per launch.
 #include "common.cuh"
-#include "pack.cuh"
 #include "camera_kernels.cuh"
 #include "rectify_kernels.cuh"
 #include "rectmath.h"
@@ -77,22 +76,18 @@ plp_status plp_undistort_keypoints(plp_ctx *ctx, const plp_camera *cam, const pl
     UndistJob J;
     PLP_TRY(make_undist_job(cam, dist, &J));
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    Packer pk;
-    const size_t o_in = pk.add(kp, (size_t)n * sizeof(plp_keypoint));
-    const size_t o_out = pk.reserve((size_t)n * sizeof(plp_keypoint));
-    const size_t o_b = pk.reserve(bearings_out ? (size_t)n * 24 : 0);
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
+    DevLayout L;
     J.batch = 1;
     J.cap = n;
-    J.kp = Packer::at<plp_keypoint>(d, o_in);
+    L.in(J.kp, kp, n);
     J.n_kp = nullptr;
-    J.out = Packer::at<plp_keypoint>(d, o_out);
-    J.bearings = bearings_out ? Packer::at<double>(d, o_b) : nullptr;
+    L.out(J.out, n);
+    J.bearings = nullptr;
+    if (bearings_out) L.out(J.bearings, (size_t)n * 3);
+    PLP_TRY(stage(ctx, 0, L));
     PLP_TRY(launch_undistort(ctx, J));
-    PLP_CUDA_TRY(cudaMemcpyAsync(undist_out, J.out, (size_t)n * sizeof(plp_keypoint), cudaMemcpyDeviceToHost, ctx->stream));
-    if (bearings_out)
-        PLP_CUDA_TRY(cudaMemcpyAsync(bearings_out, J.bearings, (size_t)n * 24, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, undist_out, J.out, n));
+    if (bearings_out) PLP_CUDA_TRY(to_host(ctx, bearings_out, J.bearings, (size_t)n * 3));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return PLP_OK;
 }

@@ -9,6 +9,7 @@
 
 #include "../../include/plpslam_b200.h"
 #include "devmath.cuh"
+#include "layout.h"
 
 namespace plp {
 
@@ -47,6 +48,17 @@ void timing_begin(plp_ctx *ctx, const char *name);
 void timing_end(plp_ctx *ctx);
 plp_status ctx_scratch(plp_ctx *ctx, int slot, size_t bytes, void **out);
 plp_status ctx_pinned(plp_ctx *ctx, size_t bytes, void **out);
+// The two backings of a DevLayout (layout.h).  stage: a call's layout in scratch slot `slot`, its inputs gathered in the
+// pinned staging buffer and sent in ONE host-to-device copy (per-array copies would be launch-latency bound at these
+// sizes).  alloc: a handle's layout in one cudaMalloc into *block, which the handle frees (null if the allocation
+// failed); `zero` clears the whole block before the inputs are copied, and the copy is waited for.
+plp_status stage(plp_ctx *ctx, int slot, DevLayout &L);
+cudaError_t alloc(plp_ctx *ctx, DevLayout &L, uint8_t **block, bool zero);
+// queues the copy of `count` elements of a device output into caller memory
+template <class T>
+cudaError_t to_host(plp_ctx *ctx, T *dst, const T *dev, size_t count) {
+    return cudaMemcpyAsync(dst, dev, count * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream);
+}
 // Opt a kernel in to the DEVICE MAXIMUM of dynamic shared memory, once per (kernel, device), and check that `need`
 // fits.  cudaFuncAttributeMaxDynamicSharedMemorySize is global per kernel: setting it to the size of the current
 // problem would lower it under a concurrent larger launch of another handle / thread, so it is only ever raised.

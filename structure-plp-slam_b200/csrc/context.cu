@@ -60,6 +60,30 @@ plp_status ctx_pinned(plp_ctx *ctx, size_t bytes, void **out) {
     return PLP_OK;
 }
 
+plp_status stage(plp_ctx *ctx, int slot, DevLayout &L) {
+    const size_t want = L.bytes() ? L.bytes() : 256;
+    void *d = nullptr, *h = nullptr;
+    PLP_TRY(ctx_scratch(ctx, slot, want, &d));
+    PLP_TRY(ctx_pinned(ctx, want, &h));
+    const size_t n = L.place((uint8_t *)d, (uint8_t *)h);
+    if (n) PLP_CUDA_TRY(cudaMemcpyAsync(d, h, n, cudaMemcpyHostToDevice, ctx->stream));
+    return PLP_OK;
+}
+
+cudaError_t alloc(plp_ctx *ctx, DevLayout &L, uint8_t **block, bool zero) {
+    cudaError_t e = cudaMalloc((void **)block, L.bytes());
+    if (e != cudaSuccess) {
+        *block = nullptr;
+        return e;
+    }
+    std::vector<uint8_t> image(L.in_bytes());
+    const size_t n = L.place(*block, image.data());
+    if (zero) e = cudaMemsetAsync(*block, 0, L.bytes(), ctx->stream);
+    if (e == cudaSuccess && n) e = cudaMemcpyAsync(*block, image.data(), n, cudaMemcpyHostToDevice, ctx->stream);
+    if (e == cudaSuccess && (zero || n)) e = cudaStreamSynchronize(ctx->stream);  // the image dies with this scope
+    return e;
+}
+
 plp_status ensure_smem_optin(const void *kernel, size_t need, const char *name) {
     static std::mutex mu;
     static std::map<std::pair<const void *, int>, size_t> done;  // (kernel, device) -> opted-in bytes

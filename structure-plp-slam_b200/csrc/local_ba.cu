@@ -27,7 +27,6 @@
 // identical and it removes all bookkeeping.  Numeric Jacobians (delta = 1e-9 central differences) are used where
 // the reference has no linearizeOplus (line edges, plane edges), see g2o BaseBinaryEdge::linearizeOplus.
 #include "common.cuh"
-#include "pack.cuh"
 #include "se3.cuh"
 #include "ba_kernels.cuh"
 #include "ba_lm_kernels.cuh"

@@ -24,38 +24,6 @@ using lm::local_gather_kernel;
 using lm::local_observe_kernel;
 using lm::local_prep_kernel;
 
-// the scratch of plp_tracker_reserve_local_map, carved from one allocation (B frames, C keypoints, ML local rows)
-struct LocalLayout {
-    size_t excl, center, qx, qy, qr, qmin, qmax, qv, choice, best, nm, claimed, mjobs, posejobs, obs, obs_kp, obs_out;
-    size_t bytes;
-    LocalLayout(size_t B, size_t C, size_t ML) {
-        size_t off = 0;
-        auto take = [&](size_t n) {
-            const size_t o = off;
-            off += (n + 255) & ~(size_t)255;
-            return o;
-        };
-        excl = take(B * ML);
-        center = take(B * 3 * 8);
-        qx = take(B * ML * 4);
-        qy = take(B * ML * 4);
-        qr = take(B * ML * 4);
-        qmin = take(B * ML * 4);
-        qmax = take(B * ML * 4);
-        qv = take(B * ML);
-        choice = take(B * ML * 4);
-        best = take(B * ML * 4);
-        nm = take(B * 4);
-        claimed = take(B * C);
-        mjobs = take(B * sizeof(PointMatchJob));
-        posejobs = take(B * sizeof(PoseJob));
-        obs = take(B * C * sizeof(plp_pt_obs));
-        obs_kp = take(B * C * 4);
-        obs_out = take(B * C);
-        bytes = off;
-    }
-};
-
 }  // namespace
 
 }  // namespace plp
@@ -76,14 +44,42 @@ plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale_factor,
         t->d_local = nullptr;
         t->max_local = 0;
     }
-    const LocalLayout lay(t->max_batch, t->cap, max_local_points);
-    if (cudaMalloc((void **)&t->d_local, lay.bytes) != cudaSuccess) {
-        t->d_local = nullptr;
-        set_error("tracker: cudaMalloc(%zu) for the local map failed", lay.bytes);
+    // the scratch of every later call, bound once (B frames, C keypoints, ML local rows)
+    const size_t B = t->max_batch, C = t->cap, ML = max_local_points;
+    auto D = std::make_shared<LocalDev>();
+    memset(D.get(), 0, sizeof(LocalDev));
+    DevLayout L;
+    L.out(D->excl, B * ML);
+    L.out(D->center, B * 3);
+    L.out(D->qx, B * ML);
+    L.out(D->qy, B * ML);
+    L.out(D->qradius, B * ML);
+    L.out(D->qmin, B * ML);
+    L.out(D->qmax, B * ML);
+    L.out(D->qvalid, B * ML);
+    L.out(D->choice, B * ML);
+    L.out(D->best, B * ML);
+    L.out(D->num_matches, B);
+    L.out(D->claimed, B * C);
+    L.out(D->mjobs, B);
+    L.out(D->posejobs, B);
+    L.out(D->obs, B * C);
+    L.out(D->obs_kp, B * C);
+    L.out(D->obs_outlier, B * C);
+    if (alloc(t->ctx, L, &t->d_local, false) != cudaSuccess) {
+        set_error("tracker: cudaMalloc(%zu) for the local map failed", L.bytes());
         return PLP_ERR_CUDA;
     }
     t->max_local = max_local_points;
-    for (int k = 0; k < 16; ++k) t->level_thr[k] = k < t->num_levels ? thr[k] : INFINITY;
+    D->cap = t->cap;
+    D->max_local = t->max_local;
+    D->cam = t->cam;
+    for (int l = 0; l < 16; ++l) {
+        D->scale_factors[l] = l < t->num_levels ? t->scale_factors[l] : 1.0f;
+        D->level_thr[l] = l < t->num_levels ? thr[l] : INFINITY;
+    }
+    D->num_levels = t->num_levels;
+    t->local = D;
     return PLP_OK;
 }
 
@@ -105,13 +101,8 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     const TrackDev &M = t->motion;
-    const LocalLayout lay(t->max_batch, t->cap, t->max_local);
-    uint8_t *d = t->d_local;
-    LocalDev D;
-    memset(&D, 0, sizeof(D));
+    LocalDev D = *t->local;
     D.batch = batch;
-    D.cap = t->cap;
-    D.max_local = t->max_local;
     D.n_kp = M.n_kp;
     D.x = M.x;
     D.y = M.y;
@@ -134,30 +125,7 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.valid = local->valid;
     D.offsets = local->offsets;
     D.last_local_idx = local->last_local_idx;
-    D.cam = t->cam;
-    for (int l = 0; l < 16; ++l) {
-        D.scale_factors[l] = l < t->num_levels ? t->scale_factors[l] : 1.0f;
-        D.level_thr[l] = t->level_thr[l];
-    }
-    D.num_levels = t->num_levels;
     D.margin = margin;
-    D.excl = d + lay.excl;
-    D.center = (double *)(d + lay.center);
-    D.qx = (float *)(d + lay.qx);
-    D.qy = (float *)(d + lay.qy);
-    D.qradius = (float *)(d + lay.qr);
-    D.qmin = (int32_t *)(d + lay.qmin);
-    D.qmax = (int32_t *)(d + lay.qmax);
-    D.qvalid = d + lay.qv;
-    D.choice = (int32_t *)(d + lay.choice);
-    D.best = (int32_t *)(d + lay.best);
-    D.num_matches = (uint32_t *)(d + lay.nm);
-    D.claimed = d + lay.claimed;
-    D.mjobs = (PointMatchJob *)(d + lay.mjobs);
-    D.posejobs = (PoseJob *)(d + lay.posejobs);
-    D.obs = (plp_pt_obs *)(d + lay.obs);
-    D.obs_kp = (int32_t *)(d + lay.obs_kp);
-    D.obs_outlier = d + lay.obs_out;
     D.matched = d_matched_out;
     D.local = d_local_out;
     D.observable = d_observable_out;

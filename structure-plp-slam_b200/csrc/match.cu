@@ -20,7 +20,6 @@
 #include "match_kernels.cuh"
 #include "point_match_kernels.cuh"
 #include "detmath.h"
-#include "pack.cuh"
 
 namespace plp {
 
@@ -589,16 +588,17 @@ plp_status plp_hamming_matrix(plp_ctx *ctx, const uint8_t *a, int na, const uint
     if (na == 0 || nb == 0) return PLP_OK;
     PLP_REQUIRE(a && b && dist_out, "null pointer");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    Packer pk;
-    const size_t oa = pk.add(a, (size_t)na * 32), ob = pk.add(b, (size_t)nb * 32);
-    const size_t oo = pk.reserve((size_t)na * nb * 2);
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
+    DevLayout L;
+    const uint8_t *da, *db;
+    uint16_t *dist;
+    L.in(da, a, (size_t)na * 32);
+    L.in(db, b, (size_t)nb * 32);
+    L.out(dist, (size_t)na * nb);
+    PLP_TRY(stage(ctx, 0, L));
     dim3 grid(div_up(nb, 32), div_up(na, 32)), block(32, 8);
-    PLP_LAUNCH(ctx, hamming_matrix_kernel, grid, block, 0, Packer::at<uint8_t>(d, oa), na, Packer::at<uint8_t>(d, ob), nb,
-               Packer::at<uint16_t>(d, oo));
+    PLP_LAUNCH(ctx, hamming_matrix_kernel, grid, block, 0, da, na, db, nb, dist);
     PLP_CHECK_LAUNCH();
-    PLP_CUDA_TRY(cudaMemcpyAsync(dist_out, d + oo, (size_t)na * nb * 2, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, dist_out, dist, (size_t)na * nb));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return PLP_OK;
 }
@@ -616,41 +616,34 @@ plp_status plp_hamming_nn(plp_ctx *ctx, const uint8_t *query, int nq, const uint
         return PLP_OK;
     }
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    Packer pk;
-    const size_t oq = pk.add(query, (size_t)nq * 32), ot = pk.add(train, (size_t)nt * 32);
-    const size_t oi = pk.reserve((size_t)nq * 4), od = pk.reserve((size_t)nq * 2);
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    PLP_LAUNCH(ctx, hamming_nn_kernel, div_up(nq * 32, 256), 256, 0, Packer::at<uint8_t>(d, oq), nq,
-               Packer::at<uint8_t>(d, ot), nt, Packer::at<int32_t>(d, oi), Packer::at<uint16_t>(d, od));
+    DevLayout L;
+    const uint8_t *dq, *dt;
+    int32_t *idx;
+    uint16_t *dist;
+    L.in(dq, query, (size_t)nq * 32);
+    L.in(dt, train, (size_t)nt * 32);
+    L.out(idx, nq);
+    L.out(dist, nq);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_LAUNCH(ctx, hamming_nn_kernel, div_up(nq * 32, 256), 256, 0, dq, nq, dt, nt, idx, dist);
     PLP_CHECK_LAUNCH();
-    PLP_CUDA_TRY(cudaMemcpyAsync(nn_idx, d + oi, (size_t)nq * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(nn_dist, d + od, (size_t)nq * 2, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, nn_idx, idx, nq));
+    PLP_CUDA_TRY(to_host(ctx, nn_dist, dist, nq));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return PLP_OK;
 }
 
-static plp_status pack_frame_points(Packer &pk, const plp_frame_points *f, PointMatchJob &J, size_t off[7]) {
+// the candidate side of a window-matcher job
+static void stage_frame_points(DevLayout &L, const plp_frame_points *f, PointMatchJob &J) {
     const size_t n = (size_t)f->n;
-    off[0] = pk.add(f->x, n * 4);
-    off[1] = pk.add(f->y, n * 4);
-    off[2] = pk.add(f->octave, n * 4);
-    off[3] = pk.add(f->angle, n * 4);
-    off[4] = pk.add(f->x_right, n * 4);
-    off[5] = pk.add(f->desc, n * 32);
-    off[6] = pk.add(f->claimed, n);
     J.n = f->n;
-    return PLP_OK;
-}
-
-static void bind_frame_points(uint8_t *d, const size_t off[7], PointMatchJob &J) {
-    J.x = Packer::at<float>(d, off[0]);
-    J.y = Packer::at<float>(d, off[1]);
-    J.octave = Packer::at<int32_t>(d, off[2]);
-    J.angle = Packer::at<float>(d, off[3]);
-    J.x_right = Packer::at<float>(d, off[4]);
-    J.desc = Packer::at<uint8_t>(d, off[5]);
-    J.claimed = Packer::at<uint8_t>(d, off[6]);
+    L.in(J.x, f->x, n);
+    L.in(J.y, f->y, n);
+    L.in(J.octave, f->octave, n);
+    L.in(J.angle, f->angle, n);
+    L.in(J.x_right, f->x_right, n);
+    L.in(J.desc, f->desc, n * 32);
+    L.in(J.claimed, f->claimed, n);
 }
 
 plp_status plp_match_frame_and_landmarks(plp_ctx *ctx, const plp_frame_points *frm, const plp_grid *grid,
@@ -679,38 +672,29 @@ plp_status plp_match_frame_and_landmarks(plp_ctx *ctx, const plp_frame_points *f
         qmin[i] = lvl - 1;
         qmax[i] = lvl;
     }
-    Packer pk;
+    DevLayout L;
     PointMatchJob J;
     memset(&J, 0, sizeof(J));
-    size_t fo[7];
-    pack_frame_points(pk, frm, J, fo);
-    const size_t o_qx = pk.add(q->reproj_x, (size_t)m * 4), o_qy = pk.add(q->reproj_y, (size_t)m * 4);
-    const size_t o_qxr = pk.add(q->x_right, (size_t)m * 4);
-    const size_t o_r = pk.add(radius.data(), (size_t)m * 4);
-    const size_t o_mn = pk.add(qmin.data(), (size_t)m * 4), o_mx = pk.add(qmax.data(), (size_t)m * 4);
-    const size_t o_qd = pk.add(q->desc, (size_t)m * 32), o_qv = pk.add(q->valid, (size_t)m);
-    const size_t o_choice = pk.reserve((size_t)m * 4), o_best = pk.reserve((size_t)m * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(PointMatchJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    bind_frame_points(d, fo, J);
+    const PointMatchJob *d_job;
+    stage_frame_points(L, frm, J);
     J.m = m;
-    J.qx = Packer::at<float>(d, o_qx);
-    J.qy = Packer::at<float>(d, o_qy);
-    J.qxr = Packer::at<float>(d, o_qxr);
-    J.qradius = Packer::at<float>(d, o_r);
-    J.qmin = Packer::at<int32_t>(d, o_mn);
-    J.qmax = Packer::at<int32_t>(d, o_mx);
-    J.qdesc = Packer::at<uint8_t>(d, o_qd);
-    J.qvalid = Packer::at<uint8_t>(d, o_qv);
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.best_idx_out = Packer::at<int32_t>(d, o_best);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_TRY(launch_point_match(ctx, Packer::at<PointMatchJob>(d, o_job), 1, frm->n, *grid, 1, lowe_ratio, 0));
+    L.in(J.qx, q->reproj_x, m);
+    L.in(J.qy, q->reproj_y, m);
+    L.in(J.qxr, q->x_right, m);
+    L.in(J.qradius, radius.data(), m);
+    L.in(J.qmin, qmin.data(), m);
+    L.in(J.qmax, qmax.data(), m);
+    L.in(J.qdesc, q->desc, (size_t)m * 32);
+    L.in(J.qvalid, q->valid, m);
+    L.out(J.choice, m);
+    L.out(J.best_idx_out, m);
+    L.out(J.num_matches, 1);
+    L.in(d_job, &J, 1);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_point_match(ctx, d_job, 1, frm->n, *grid, 1, lowe_ratio, 0));
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(best_idx_out, d + o_best, (size_t)m * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, best_idx_out, J.best_idx_out, m));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
@@ -734,91 +718,71 @@ plp_status plp_match_current_and_last_frames(plp_ctx *ctx, const plp_frame_point
     for (int i = 0; i < last->n; ++i) PLP_REQUIRE(last->octave[i] >= 0 && last->octave[i] < num_levels, "octave range");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     const int m = last->n, n = curr->n;
-    Packer pk;
+    DevLayout L;
     PointMatchJob J;
     memset(&J, 0, sizeof(J));
     ProjectJob P;
     memset(&P, 0, sizeof(P));
-    size_t fo[7];
-    pack_frame_points(pk, curr, J, fo);
-    const size_t o_pw = pk.add(last->pos_w, (size_t)m * 24), o_oct = pk.add(last->octave, (size_t)m * 4);
-    const size_t o_ang = pk.add(last->angle, (size_t)m * 4), o_qd = pk.add(last->desc, (size_t)m * 32);
-    const size_t o_val = pk.add(last->valid, (size_t)m);
-    const size_t o_sf = pk.add(scale_factors, (size_t)num_levels * 4);
-    const size_t o_qx = pk.reserve((size_t)m * 4), o_qy = pk.reserve((size_t)m * 4), o_qxr = pk.reserve((size_t)m * 4);
-    const size_t o_r = pk.reserve((size_t)m * 4), o_mn = pk.reserve((size_t)m * 4), o_mx = pk.reserve((size_t)m * 4);
-    const size_t o_qv = pk.reserve((size_t)m);
-    const size_t o_choice = pk.reserve((size_t)m * 4), o_matched = pk.reserve((size_t)n * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(PointMatchJob)), o_pjob = pk.reserve(sizeof(ProjectJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    bind_frame_points(d, fo, J);
+    const PointMatchJob *d_job;
+    const ProjectJob *d_pjob;
+    const float *d_sf;
+    stage_frame_points(L, curr, J);
     P.n_last = m;
-    P.pos_w = Packer::at<double>(d, o_pw);
-    P.octave = Packer::at<int32_t>(d, o_oct);
-    P.valid = Packer::at<uint8_t>(d, o_val);
+    L.in(P.pos_w, last->pos_w, (size_t)m * 3);
+    L.in(P.octave, last->octave, m);
+    L.in(J.qangle, last->angle, m);
+    L.in(J.qdesc, last->desc, (size_t)m * 32);
+    L.in(P.valid, last->valid, m);
+    L.in(d_sf, scale_factors, num_levels);
     for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 4; ++c) P.pose_cw[r * 4 + c] = pose_cw_curr[r * 4 + c];
     motion_assumption(*cam, pose_cw_curr, pose_cw_last, &P.assume_forward, &P.assume_backward);
-    P.qx = Packer::at<float>(d, o_qx);
-    P.qy = Packer::at<float>(d, o_qy);
-    P.qxr = Packer::at<float>(d, o_qxr);
-    P.qradius = Packer::at<float>(d, o_r);
-    P.qmin = Packer::at<int32_t>(d, o_mn);
-    P.qmax = Packer::at<int32_t>(d, o_mx);
-    P.qvalid = Packer::at<uint8_t>(d, o_qv);
+    // the reprojection pre-pass writes the queries the matcher reads
+    L.out(P.qx, m);
+    L.out(P.qy, m);
+    L.out(P.qxr, m);
+    L.out(P.qradius, m);
+    L.out(P.qmin, m);
+    L.out(P.qmax, m);
+    L.out(P.qvalid, m);
     J.m = m;
-    J.qx = P.qx;
-    J.qy = P.qy;
-    J.qxr = P.qxr;
-    J.qradius = P.qradius;
-    J.qmin = P.qmin;
-    J.qmax = P.qmax;
-    J.qangle = Packer::at<float>(d, o_ang);
-    J.qdesc = Packer::at<uint8_t>(d, o_qd);
-    J.qvalid = P.qvalid;
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.matched_out = Packer::at<int32_t>(d, o_matched);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_pjob, &P, sizeof(P), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_TRY(launch_project_points(ctx, Packer::at<ProjectJob>(d, o_pjob), 1, m, *cam, Packer::at<float>(d, o_sf),
-                                  num_levels, margin));
-    PLP_TRY(launch_point_match(ctx, Packer::at<PointMatchJob>(d, o_job), 1, n, *grid, 0, 0.0f, check_orientation));
+    L.same(J.qx, P.qx);
+    L.same(J.qy, P.qy);
+    L.same(J.qxr, P.qxr);
+    L.same(J.qradius, P.qradius);
+    L.same(J.qmin, P.qmin);
+    L.same(J.qmax, P.qmax);
+    L.same(J.qvalid, P.qvalid);
+    L.out(J.choice, m);
+    L.out(J.matched_out, n);
+    L.out(J.num_matches, 1);
+    L.in(d_job, &J, 1);
+    L.in(d_pjob, &P, 1);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_project_points(ctx, d_pjob, 1, m, *cam, d_sf, num_levels, margin));
+    PLP_TRY(launch_point_match(ctx, d_job, 1, n, *grid, 0, 0.0f, check_orientation));
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(matched_last_idx_out, d + o_matched, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, matched_last_idx_out, J.matched_out, n));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
 }
 
-static void pack_frame_lines(Packer &pk, const plp_frame_lines *f, size_t off[11]) {
+// the candidate side of a keyline-matcher job
+static void stage_frame_lines(DevLayout &L, const plp_frame_lines *f, LineMatchJob &J) {
     const size_t n = (size_t)f->n;
-    off[0] = pk.add(f->sx, n * 4);
-    off[1] = pk.add(f->sy, n * 4);
-    off[2] = pk.add(f->ex, n * 4);
-    off[3] = pk.add(f->ey, n * 4);
-    off[4] = pk.add(f->octave, n * 4);
-    off[5] = pk.add(f->ratio_level, n * 4);
-    off[6] = pk.add(f->x_right_sp, n * 4);
-    off[7] = pk.add(f->x_right_ep, n * 4);
-    off[8] = pk.add(f->desc, n * 32);
-    off[9] = pk.add(f->claimed, n);
-}
-
-static void bind_frame_lines(uint8_t *d, const size_t off[11], const plp_frame_lines *f, LineMatchJob &J) {
     J.n = f->n;
-    J.sx = Packer::at<float>(d, off[0]);
-    J.sy = Packer::at<float>(d, off[1]);
-    J.ex = Packer::at<float>(d, off[2]);
-    J.ey = Packer::at<float>(d, off[3]);
-    J.octave = Packer::at<int32_t>(d, off[4]);
-    J.ratio_level = Packer::at<int32_t>(d, off[5]);
-    J.xr_sp = Packer::at<float>(d, off[6]);
-    J.xr_ep = Packer::at<float>(d, off[7]);
-    J.desc = Packer::at<uint8_t>(d, off[8]);
-    J.claimed = Packer::at<uint8_t>(d, off[9]);
+    L.in(J.sx, f->sx, n);
+    L.in(J.sy, f->sy, n);
+    L.in(J.ex, f->ex, n);
+    L.in(J.ey, f->ey, n);
+    L.in(J.octave, f->octave, n);
+    L.in(J.ratio_level, f->ratio_level, n);
+    L.in(J.xr_sp, f->x_right_sp, n);
+    L.in(J.xr_ep, f->x_right_ep, n);
+    L.in(J.desc, f->desc, n * 32);
+    L.in(J.claimed, f->claimed, n);
 }
 
 plp_status plp_match_frame_and_landmarks_line(plp_ctx *ctx, const plp_frame_lines *frm, const float *scale_factors_lsd,
@@ -846,39 +810,30 @@ plp_status plp_match_frame_and_landmarks_line(plp_ctx *ctx, const plp_frame_line
         qmin[i] = lvl - 1;
         qmax[i] = lvl;
     }
-    Packer pk;
+    DevLayout L;
     LineMatchJob J;
     memset(&J, 0, sizeof(J));
-    size_t fo[11];
-    pack_frame_lines(pk, frm, fo);
-    const size_t o1 = pk.add(q->sp_x, (size_t)m * 4), o2 = pk.add(q->sp_y, (size_t)m * 4);
-    const size_t o3 = pk.add(q->ep_x, (size_t)m * 4), o4 = pk.add(q->ep_y, (size_t)m * 4);
-    const size_t o_r = pk.add(radius.data(), (size_t)m * 4);
-    const size_t o_mn = pk.add(qmin.data(), (size_t)m * 4), o_mx = pk.add(qmax.data(), (size_t)m * 4);
-    const size_t o_qd = pk.add(q->desc, (size_t)m * 32), o_qv = pk.add(q->valid, (size_t)m);
-    const size_t o_choice = pk.reserve((size_t)m * 4), o_best = pk.reserve((size_t)m * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(LineMatchJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    bind_frame_lines(d, fo, frm, J);
+    const LineMatchJob *d_job;
+    stage_frame_lines(L, frm, J);
     J.m = m;
-    J.q_spx = Packer::at<float>(d, o1);
-    J.q_spy = Packer::at<float>(d, o2);
-    J.q_epx = Packer::at<float>(d, o3);
-    J.q_epy = Packer::at<float>(d, o4);
-    J.qradius = Packer::at<float>(d, o_r);
-    J.qmin = Packer::at<int32_t>(d, o_mn);
-    J.qmax = Packer::at<int32_t>(d, o_mx);
-    J.qdesc = Packer::at<uint8_t>(d, o_qd);
-    J.qvalid = Packer::at<uint8_t>(d, o_qv);
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.best_idx_out = Packer::at<int32_t>(d, o_best);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_TRY(launch_line_match(ctx, Packer::at<LineMatchJob>(d, o_job), 1, 1, lowe_ratio, 0));
+    L.in(J.q_spx, q->sp_x, m);
+    L.in(J.q_spy, q->sp_y, m);
+    L.in(J.q_epx, q->ep_x, m);
+    L.in(J.q_epy, q->ep_y, m);
+    L.in(J.qradius, radius.data(), m);
+    L.in(J.qmin, qmin.data(), m);
+    L.in(J.qmax, qmax.data(), m);
+    L.in(J.qdesc, q->desc, (size_t)m * 32);
+    L.in(J.qvalid, q->valid, m);
+    L.out(J.choice, m);
+    L.out(J.best_idx_out, m);
+    L.out(J.num_matches, 1);
+    L.in(d_job, &J, 1);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_line_match(ctx, d_job, 1, 1, lowe_ratio, 0));
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(best_idx_out, d + o_best, (size_t)m * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, best_idx_out, J.best_idx_out, m));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
@@ -904,66 +859,59 @@ plp_status plp_match_current_and_last_frames_line(plp_ctx *ctx, const plp_frame_
         PLP_REQUIRE(last->octave[i] >= 0 && last->octave[i] < num_levels_lsd, "octave range");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     const int m = last->n, n = curr->n;
-    Packer pk;
+    DevLayout L;
     LineMatchJob J;
     memset(&J, 0, sizeof(J));
     ProjectJob P;
     memset(&P, 0, sizeof(P));
-    size_t fo[11];
-    pack_frame_lines(pk, curr, fo);
-    const size_t o_pw = pk.add(last->pos_w, (size_t)m * 48), o_oct = pk.add(last->octave, (size_t)m * 4);
-    const size_t o_qd = pk.add(last->desc, (size_t)m * 32), o_val = pk.add(last->valid, (size_t)m);
-    const size_t o_sf = pk.add(scale_factors_lsd, (size_t)num_levels_lsd * 4);
-    size_t oq[6];
-    for (int k = 0; k < 6; ++k) oq[k] = pk.reserve((size_t)m * 4);
-    const size_t o_r = pk.reserve((size_t)m * 4), o_mn = pk.reserve((size_t)m * 4), o_mx = pk.reserve((size_t)m * 4);
-    const size_t o_qv = pk.reserve((size_t)m);
-    const size_t o_choice = pk.reserve((size_t)m * 4), o_matched = pk.reserve((size_t)n * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(LineMatchJob)), o_pjob = pk.reserve(sizeof(ProjectJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    bind_frame_lines(d, fo, curr, J);
+    const LineMatchJob *d_job;
+    const ProjectJob *d_pjob;
+    const float *d_sf;
+    plp_frame_lines frame = *curr;
+    frame.ratio_level = nullptr;  // the octave decides the ratio level
+    stage_frame_lines(L, &frame, J);
     P.n_last = m;
-    P.pos_w = Packer::at<double>(d, o_pw);
-    P.octave = Packer::at<int32_t>(d, o_oct);
-    P.valid = Packer::at<uint8_t>(d, o_val);
+    L.in(P.pos_w, last->pos_w, (size_t)m * 6);
+    L.in(P.octave, last->octave, m);
+    L.in(J.qdesc, last->desc, (size_t)m * 32);
+    L.in(P.valid, last->valid, m);
+    L.in(d_sf, scale_factors_lsd, num_levels_lsd);
     for (int r = 0; r < 3; ++r)
         for (int c = 0; c < 4; ++c) P.pose_cw[r * 4 + c] = pose_cw_curr[r * 4 + c];
     motion_assumption(*cam, pose_cw_curr, pose_cw_last, &P.assume_forward, &P.assume_backward);
-    P.qx = Packer::at<float>(d, oq[0]);
-    P.qy = Packer::at<float>(d, oq[1]);
-    P.qxr = Packer::at<float>(d, oq[2]);
-    P.qx2 = Packer::at<float>(d, oq[3]);
-    P.qy2 = Packer::at<float>(d, oq[4]);
-    P.qxr2 = Packer::at<float>(d, oq[5]);
-    P.qradius = Packer::at<float>(d, o_r);
-    P.qmin = Packer::at<int32_t>(d, o_mn);
-    P.qmax = Packer::at<int32_t>(d, o_mx);
-    P.qvalid = Packer::at<uint8_t>(d, o_qv);
+    // the reprojection pre-pass writes the queries the matcher reads
+    L.out(P.qx, m);
+    L.out(P.qy, m);
+    L.out(P.qxr, m);
+    L.out(P.qx2, m);
+    L.out(P.qy2, m);
+    L.out(P.qxr2, m);
+    L.out(P.qradius, m);
+    L.out(P.qmin, m);
+    L.out(P.qmax, m);
+    L.out(P.qvalid, m);
     J.m = m;
-    J.q_spx = P.qx;
-    J.q_spy = P.qy;
-    J.q_xr_sp = P.qxr;
-    J.q_epx = P.qx2;
-    J.q_epy = P.qy2;
-    J.q_xr_ep = P.qxr2;
-    J.qradius = P.qradius;
-    J.qmin = P.qmin;
-    J.qmax = P.qmax;
-    J.qdesc = Packer::at<uint8_t>(d, o_qd);
-    J.qvalid = P.qvalid;
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.matched_out = Packer::at<int32_t>(d, o_matched);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
-    J.ratio_level = nullptr;
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_pjob, &P, sizeof(P), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_TRY(launch_project_lines(ctx, Packer::at<ProjectJob>(d, o_pjob), 1, m, *cam, Packer::at<float>(d, o_sf),
-                                 num_levels_lsd, margin));
-    PLP_TRY(launch_line_match(ctx, Packer::at<LineMatchJob>(d, o_job), 1, 0, 0.0f, cam->setup_type == 2));
+    L.same(J.q_spx, P.qx);
+    L.same(J.q_spy, P.qy);
+    L.same(J.q_xr_sp, P.qxr);
+    L.same(J.q_epx, P.qx2);
+    L.same(J.q_epy, P.qy2);
+    L.same(J.q_xr_ep, P.qxr2);
+    L.same(J.qradius, P.qradius);
+    L.same(J.qmin, P.qmin);
+    L.same(J.qmax, P.qmax);
+    L.same(J.qvalid, P.qvalid);
+    L.out(J.choice, m);
+    L.out(J.matched_out, n);
+    L.out(J.num_matches, 1);
+    L.in(d_job, &J, 1);
+    L.in(d_pjob, &P, 1);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_project_lines(ctx, d_pjob, 1, m, *cam, d_sf, num_levels_lsd, margin));
+    PLP_TRY(launch_line_match(ctx, d_job, 1, 0, 0.0f, cam->setup_type == 2));
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(matched_last_idx_out, d + o_matched, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, matched_last_idx_out, J.matched_out, n));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
@@ -993,41 +941,32 @@ plp_status plp_match_frame_and_keyframe(plp_ctx *ctx, const plp_frame_points *fr
         qmin[i] = lvl - 1;
         qmax[i] = lvl + 1;
     }
-    Packer pk;
+    DevLayout L;
     PointMatchJob J;
     memset(&J, 0, sizeof(J));
-    size_t fo[7];
-    pack_frame_points(pk, frm, J, fo);
-    const size_t o_qx = pk.add(q->reproj_x, (size_t)m * 4), o_qy = pk.add(q->reproj_y, (size_t)m * 4);
-    const size_t o_r = pk.add(radius.data(), (size_t)m * 4);
-    const size_t o_mn = pk.add(qmin.data(), (size_t)m * 4), o_mx = pk.add(qmax.data(), (size_t)m * 4);
-    const size_t o_qa = pk.add(q_angle, (size_t)m * 4);
-    const size_t o_qd = pk.add(q->desc, (size_t)m * 32), o_qv = pk.add(q->valid, (size_t)m);
-    const size_t o_choice = pk.reserve((size_t)m * 4), o_matched = pk.reserve((size_t)n * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(PointMatchJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    bind_frame_points(d, fo, J);
-    J.x_right = nullptr;  // no stereo gate in match_frame_and_keyframe
+    const PointMatchJob *d_job;
+    plp_frame_points frame = *frm;
+    frame.x_right = nullptr;  // no stereo gate in match_frame_and_keyframe
+    stage_frame_points(L, &frame, J);
     J.m = m;
-    J.qx = Packer::at<float>(d, o_qx);
-    J.qy = Packer::at<float>(d, o_qy);
-    J.qxr = nullptr;
-    J.qradius = Packer::at<float>(d, o_r);
-    J.qmin = Packer::at<int32_t>(d, o_mn);
-    J.qmax = Packer::at<int32_t>(d, o_mx);
-    J.qangle = q_angle ? Packer::at<float>(d, o_qa) : nullptr;
-    J.qdesc = Packer::at<uint8_t>(d, o_qd);
-    J.qvalid = q->valid ? Packer::at<uint8_t>(d, o_qv) : nullptr;
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.matched_out = Packer::at<int32_t>(d, o_matched);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
+    L.in(J.qx, q->reproj_x, m);
+    L.in(J.qy, q->reproj_y, m);
+    L.in(J.qradius, radius.data(), m);
+    L.in(J.qmin, qmin.data(), m);
+    L.in(J.qmax, qmax.data(), m);
+    L.in(J.qangle, q_angle, m);
+    L.in(J.qdesc, q->desc, (size_t)m * 32);
+    L.in(J.qvalid, q->valid, m);
+    L.out(J.choice, m);
+    L.out(J.matched_out, n);
+    L.out(J.num_matches, 1);
     J.hamm_thr_p1 = hamm_dist_thr + 1u;
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_TRY(launch_point_match(ctx, Packer::at<PointMatchJob>(d, o_job), 1, n, *grid, 0, 0.0f, check_orientation));
+    L.in(d_job, &J, 1);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_point_match(ctx, d_job, 1, n, *grid, 0, 0.0f, check_orientation));
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(matched_kf_idx_out, d + o_matched, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, matched_kf_idx_out, J.matched_out, n));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
@@ -1056,41 +995,33 @@ plp_status plp_match_frame_and_keyframe_line(plp_ctx *ctx, const plp_frame_lines
         qmin[i] = lvl - 1;
         qmax[i] = lvl + 1;
     }
-    Packer pk;
+    DevLayout L;
     LineMatchJob J;
     memset(&J, 0, sizeof(J));
-    size_t fo[11];
-    pack_frame_lines(pk, frm, fo);
-    const size_t o1 = pk.add(q->sp_x, (size_t)m * 4), o2 = pk.add(q->sp_y, (size_t)m * 4);
-    const size_t o3 = pk.add(q->ep_x, (size_t)m * 4), o4 = pk.add(q->ep_y, (size_t)m * 4);
-    const size_t o_r = pk.add(radius.data(), (size_t)m * 4);
-    const size_t o_mn = pk.add(qmin.data(), (size_t)m * 4), o_mx = pk.add(qmax.data(), (size_t)m * 4);
-    const size_t o_qd = pk.add(q->desc, (size_t)m * 32), o_qv = pk.add(q->valid, (size_t)m);
-    const size_t o_choice = pk.reserve((size_t)m * 4), o_matched = pk.reserve((size_t)n * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(LineMatchJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    bind_frame_lines(d, fo, frm, J);
+    const LineMatchJob *d_job;
+    plp_frame_lines frame = *frm;
+    frame.ratio_level = nullptr;  // the octave decides the ratio level
+    stage_frame_lines(L, &frame, J);
     J.m = m;
-    J.q_spx = Packer::at<float>(d, o1);
-    J.q_spy = Packer::at<float>(d, o2);
-    J.q_epx = Packer::at<float>(d, o3);
-    J.q_epy = Packer::at<float>(d, o4);
-    J.qradius = Packer::at<float>(d, o_r);
-    J.qmin = Packer::at<int32_t>(d, o_mn);
-    J.qmax = Packer::at<int32_t>(d, o_mx);
-    J.qdesc = Packer::at<uint8_t>(d, o_qd);
-    J.qvalid = q->valid ? Packer::at<uint8_t>(d, o_qv) : nullptr;
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.matched_out = Packer::at<int32_t>(d, o_matched);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
-    J.ratio_level = nullptr;
+    L.in(J.q_spx, q->sp_x, m);
+    L.in(J.q_spy, q->sp_y, m);
+    L.in(J.q_epx, q->ep_x, m);
+    L.in(J.q_epy, q->ep_y, m);
+    L.in(J.qradius, radius.data(), m);
+    L.in(J.qmin, qmin.data(), m);
+    L.in(J.qmax, qmax.data(), m);
+    L.in(J.qdesc, q->desc, (size_t)m * 32);
+    L.in(J.qvalid, q->valid, m);
+    L.out(J.choice, m);
+    L.out(J.matched_out, n);
+    L.out(J.num_matches, 1);
     J.hamm_thr_p1 = hamm_dist_thr + 1u;
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_TRY(launch_line_match(ctx, Packer::at<LineMatchJob>(d, o_job), 1, 0, 0.0f, 0));
+    L.in(d_job, &J, 1);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_line_match(ctx, d_job, 1, 0, 0.0f, 0));
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(matched_kf_idx_out, d + o_matched, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, matched_kf_idx_out, J.matched_out, n));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
@@ -1108,32 +1039,26 @@ plp_status plp_match_brute_force(plp_ctx *ctx, const uint8_t *frm_desc, const fl
     PLP_REQUIRE(frm_desc && kf_desc, "descriptors");
     PLP_REQUIRE(!check_orientation || (frm_angle && kf_angle), "angles required for the orientation check");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    Packer pk;
+    DevLayout L;
     BruteJob J;
     memset(&J, 0, sizeof(J));
-    const size_t o1 = pk.add(frm_desc, (size_t)n_frm * 32), o2 = pk.add(frm_angle, (size_t)n_frm * 4);
-    const size_t o3 = pk.add(kf_desc, (size_t)n_kf * 32), o4 = pk.add(kf_angle, (size_t)n_kf * 4);
-    const size_t o5 = pk.add(kf_valid, (size_t)n_kf);
-    const size_t o_choice = pk.reserve((size_t)n_kf * 4), o_matched = pk.reserve((size_t)n_frm * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(BruteJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
+    const BruteJob *d_job;
     J.n_frm = n_frm;
-    J.frm_desc = Packer::at<uint8_t>(d, o1);
-    J.frm_angle = Packer::at<float>(d, o2);
+    L.in(J.frm_desc, frm_desc, (size_t)n_frm * 32);
+    L.in(J.frm_angle, frm_angle, n_frm);
     J.n_kf = n_kf;
-    J.kf_desc = Packer::at<uint8_t>(d, o3);
-    J.kf_angle = Packer::at<float>(d, o4);
-    J.kf_valid = Packer::at<uint8_t>(d, o5);
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.matched_out = Packer::at<int32_t>(d, o_matched);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
-    PLP_TRY(launch_brute_match(ctx, Packer::at<BruteJob>(d, o_job), 1, n_frm, lowe_ratio, check_orientation));
+    L.in(J.kf_desc, kf_desc, (size_t)n_kf * 32);
+    L.in(J.kf_angle, kf_angle, n_kf);
+    L.in(J.kf_valid, kf_valid, n_kf);
+    L.out(J.choice, n_kf);
+    L.out(J.matched_out, n_frm);
+    L.out(J.num_matches, 1);
+    L.in(d_job, &J, 1);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_TRY(launch_brute_match(ctx, d_job, 1, n_frm, lowe_ratio, check_orientation));
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(matched_kf_idx_in_frm_out, d + o_matched, (size_t)n_frm * 4, cudaMemcpyDeviceToHost,
-                                 ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, matched_kf_idx_in_frm_out, J.matched_out, n_frm));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
@@ -1193,53 +1118,42 @@ plp_status plp_match_for_triangulation(plp_ctx *ctx, const plp_keyframe_points *
         for (size_t i = 0; i < n1; ++i) st1[i] = 0 <= kf1->x_right[i];
     if (kf2->x_right)
         for (size_t i = 0; i < n2; ++i) st2[i] = 0 <= kf2->x_right[i];
-    Packer pk;
+    DevLayout L;
     TriJob J;
     memset(&J, 0, sizeof(J));
-    const size_t o_d1 = pk.add(kf1->desc, n1 * 32), o_d2 = pk.add(kf2->desc, n2 * 32);
-    const size_t o_a1 = pk.add(kf1->angle, n1 * 4), o_a2 = pk.add(kf2->angle, n2 * 4);
-    const size_t o_o1 = pk.add(kf1->octave, n1 * 4);
-    const size_t o_b1 = pk.add(kf1->bearings, n1 * 24), o_b2 = pk.add(kf2->bearings, n2 * 24);
-    const size_t o_l2 = pk.add(kf2->has_landmark, n2);
-    const size_t o_s1 = pk.add(st1.data(), n1), o_s2 = pk.add(st2.data(), n2);
-    const size_t o_q1 = pk.add(seq_idx1.data(), (size_t)P * 4), o_qb = pk.add(seq_cbeg.data(), (size_t)P * 4);
-    const size_t o_qe = pk.add(seq_cend.data(), (size_t)P * 4), o_c2 = pk.add(cand2.data(), cand2.size() * 4);
-    const size_t o_sf = pk.add(scale_factors_1, (size_t)num_levels * 4);
-    const size_t o_choice = pk.reserve((size_t)P * 4), o_matched = pk.reserve(n1 * 4), o_num = pk.reserve(4);
-    const size_t o_job = pk.reserve(sizeof(TriJob));
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
+    const TriJob *d_job;
     J.n1 = (int)n1;
     J.n2 = (int)n2;
     J.num_seq = P;
-    J.desc1 = Packer::at<uint8_t>(d, o_d1);
-    J.desc2 = Packer::at<uint8_t>(d, o_d2);
-    J.angle1 = kf1->angle ? Packer::at<float>(d, o_a1) : nullptr;
-    J.angle2 = kf2->angle ? Packer::at<float>(d, o_a2) : nullptr;
-    J.octave1 = Packer::at<int32_t>(d, o_o1);
-    J.bearing1 = Packer::at<double>(d, o_b1);
-    J.bearing2 = Packer::at<double>(d, o_b2);
-    J.has_lm2 = Packer::at<uint8_t>(d, o_l2);
-    J.stereo1 = Packer::at<uint8_t>(d, o_s1);
-    J.stereo2 = Packer::at<uint8_t>(d, o_s2);
-    J.seq_idx1 = Packer::at<int32_t>(d, o_q1);
-    J.seq_cbeg = Packer::at<int32_t>(d, o_qb);
-    J.seq_cend = Packer::at<int32_t>(d, o_qe);
-    J.cand2 = Packer::at<int32_t>(d, o_c2);
-    J.scale_factors1 = Packer::at<float>(d, o_sf);
+    L.in(J.desc1, kf1->desc, n1 * 32);
+    L.in(J.desc2, kf2->desc, n2 * 32);
+    L.in(J.angle1, kf1->angle, n1);
+    L.in(J.angle2, kf2->angle, n2);
+    L.in(J.octave1, kf1->octave, n1);
+    L.in(J.bearing1, kf1->bearings, n1 * 3);
+    L.in(J.bearing2, kf2->bearings, n2 * 3);
+    L.in(J.has_lm2, kf2->has_landmark, n2);
+    L.in(J.stereo1, st1.data(), n1);
+    L.in(J.stereo2, st2.data(), n2);
+    L.in(J.seq_idx1, seq_idx1.data(), P);
+    L.in(J.seq_cbeg, seq_cbeg.data(), P);
+    L.in(J.seq_cend, seq_cend.data(), P);
+    L.in(J.cand2, cand2.data(), cand2.size());
+    L.in(J.scale_factors1, scale_factors_1, num_levels);
     for (int k = 0; k < 9; ++k) J.E[k] = E_12[k];
     for (int k = 0; k < 3; ++k) J.epipole[k] = epipole_bearing_in_2[k];
-    J.choice = Packer::at<int32_t>(d, o_choice);
-    J.matched_out = Packer::at<int32_t>(d, o_matched);
-    J.num_matches = Packer::at<uint32_t>(d, o_num);
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_job, &J, sizeof(J), cudaMemcpyHostToDevice, ctx->stream));
+    L.out(J.choice, P);
+    L.out(J.matched_out, n1);
+    L.out(J.num_matches, 1);
+    L.in(d_job, &J, 1);
+    PLP_TRY(stage(ctx, 0, L));
     const size_t smem = (size_t)n2 * 8 + (kHistLen + 4) * 4 + kHistLen + 16;
     PLP_SMEM_OPTIN(triangulation_match_kernel, smem);
-    PLP_LAUNCH(ctx, triangulation_match_kernel, 1, kThreads, smem, Packer::at<TriJob>(d, o_job), (int)n2, check_orientation);
+    PLP_LAUNCH(ctx, triangulation_match_kernel, 1, kThreads, smem, d_job, (int)n2, check_orientation);
     PLP_CHECK_LAUNCH();
     uint32_t num = 0;
-    PLP_CUDA_TRY(cudaMemcpyAsync(matched_idx2_in_1_out, d + o_matched, n1 * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(&num, d + o_num, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, matched_idx2_in_1_out, J.matched_out, n1));
+    PLP_CUDA_TRY(to_host(ctx, &num, J.num_matches, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     if (num_matches_out) *num_matches_out = num;
     return PLP_OK;
@@ -1254,15 +1168,18 @@ plp_status plp_landmark_compute_descriptor_batch(plp_ctx *ctx, const uint8_t *de
     PLP_REQUIRE(offsets[0] == 0 && total >= 0 && (total == 0 || descs), "offsets");
     for (int i = 0; i < num_landmarks; ++i) PLP_REQUIRE(offsets[i] <= offsets[i + 1], "offsets must ascend");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    Packer pk;
-    const size_t o_d = pk.add(descs, (size_t)total * 32), o_o = pk.add(offsets, (size_t)(num_landmarks + 1) * 4);
-    const size_t o_b = pk.reserve((size_t)num_landmarks * 4);
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
-    PLP_LAUNCH(ctx, median_descriptor_kernel, div_up(num_landmarks, kMedWarps), kMedWarps * 32, 0, Packer::at<uint8_t>(d, o_d),
-               Packer::at<int32_t>(d, o_o), num_landmarks, Packer::at<int32_t>(d, o_b));
+    DevLayout L;
+    const uint8_t *d_descs;
+    const int32_t *d_offsets;
+    int32_t *d_best;
+    L.in(d_descs, descs, (size_t)total * 32);
+    L.in(d_offsets, offsets, (size_t)num_landmarks + 1);
+    L.out(d_best, num_landmarks);
+    PLP_TRY(stage(ctx, 0, L));
+    PLP_LAUNCH(ctx, median_descriptor_kernel, div_up(num_landmarks, kMedWarps), kMedWarps * 32, 0, d_descs, d_offsets,
+               num_landmarks, d_best);
     PLP_CHECK_LAUNCH();
-    PLP_CUDA_TRY(cudaMemcpyAsync(best_idx_out, d + o_b, (size_t)num_landmarks * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, best_idx_out, d_best, num_landmarks));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return PLP_OK;
 }

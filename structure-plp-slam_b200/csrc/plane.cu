@@ -5,7 +5,6 @@
 // landmarks, thread 0 compacts the inliers in index order and refits), then a one-CTA kernel replays the reference's
 // sequential bookkeeping over the per-hypothesis results and applies step [4].  FP64, compiled with -fmad=false.
 #include "common.cuh"
-#include "pack.cuh"
 #include "plane_kernels.cuh"
 
 
@@ -36,44 +35,37 @@ plp_status plp_plane_ransac(plp_ctx *ctx, const double *pos_w, const uint8_t *va
     for (long long i = 0; i < (long long)num_iter * sample_size; ++i)
         PLP_REQUIRE(samples[i] >= 0 && samples[i] < n, "sample index out of range");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    Packer pk;
+    DevLayout L;
     const size_t N = (size_t)n, K = (size_t)num_iter;
-    const size_t o_pos = pk.add(pos_w, N * 24), o_val = pk.add(valid, N);
-    const size_t o_smp = pk.add(samples, K * (size_t)sample_size * 4);
-    const size_t o_eq = pk.add(eq_inout, 32), o_pe = pk.add(plane_error_inout, 8);
-    const size_t o_eqs = pk.reserve(K * 32), o_eqr = pk.reserve(K * 32), o_res = pk.reserve(K * 8), o_err = pk.reserve(K * 8);
-    const size_t o_el = pk.reserve(K * 4), o_cnt = pk.reserve(K * 4), o_flag = pk.reserve(K * N), o_idx = pk.reserve(K * N * 4);
-    const size_t o_inl = pk.reserve(N), o_st = pk.reserve(4);
-    uint8_t *d;
-    PLP_TRY(pk.upload(ctx, 0, &d));
     PlaneJob J;
-    J.pos = Packer::at<double>(d, o_pos);
-    J.valid = Packer::at<uint8_t>(d, o_val);
-    J.samples = Packer::at<int32_t>(d, o_smp);
+    L.in(J.pos, pos_w, N * 3);
+    L.in(J.valid, valid, N);
+    L.in(J.samples, samples, K * (size_t)sample_size);
+    L.in(J.eq, eq_inout, 4);
+    L.in(J.plane_err, plane_error_inout, 1);
     J.n = n;
     J.num_iter = num_iter;
     J.sample_size = sample_size;
     J.cfg = *cfg;
-    J.eq_s = Packer::at<double>(d, o_eqs);
-    J.eq_r = Packer::at<double>(d, o_eqr);
-    J.res = Packer::at<double>(d, o_res);
-    J.err = Packer::at<double>(d, o_err);
-    J.elig = Packer::at<int32_t>(d, o_el);
-    J.cnt = Packer::at<int32_t>(d, o_cnt);
-    J.flag = Packer::at<uint8_t>(d, o_flag);
-    J.idx = Packer::at<int32_t>(d, o_idx);
-    J.eq = Packer::at<double>(d, o_eq);
-    J.plane_err = Packer::at<double>(d, o_pe);
-    J.inlier = Packer::at<uint8_t>(d, o_inl);
-    J.status = Packer::at<int32_t>(d, o_st);
+    L.out(J.eq_s, K * 4);
+    L.out(J.eq_r, K * 4);
+    L.out(J.res, K);
+    L.out(J.err, K);
+    L.out(J.elig, K);
+    L.out(J.cnt, K);
+    L.out(J.flag, K * N);
+    L.out(J.idx, K * N);
+    L.out(J.inlier, N);
+    L.out(J.status, 1);
+    PLP_TRY(stage(ctx, 0, L));
     PLP_LAUNCH(ctx, plane_hypothesis_kernel, num_iter, kPlThreads, 0, J);
     PLP_CHECK_LAUNCH();
     PLP_LAUNCH(ctx, plane_select_kernel, 1, kPlThreads, 0, J);
     PLP_CHECK_LAUNCH();
-    PLP_CUDA_TRY(cudaMemcpyAsync(eq_inout, d + o_eq, 32, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(plane_error_inout, d + o_pe, 8, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(inlier_out, d + o_inl, N, cudaMemcpyDeviceToHost, ctx->stream));
-    PLP_CUDA_TRY(cudaMemcpyAsync(status_out, d + o_st, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_CUDA_TRY(to_host(ctx, eq_inout, J.eq, 4));
+    PLP_CUDA_TRY(to_host(ctx, plane_error_inout, J.plane_err, 1));
+    PLP_CUDA_TRY(to_host(ctx, inlier_out, J.inlier, N));
+    PLP_CUDA_TRY(to_host(ctx, status_out, J.status, 1));
     PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return PLP_OK;
 }

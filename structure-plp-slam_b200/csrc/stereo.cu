@@ -289,26 +289,29 @@ plp_status plp_stereo_compute(plp_ctx *ctx, const plp_orb *left, const plp_orb *
     const int cap = plp_orb_capacity(left);
     PLP_REQUIRE(n_l <= cap && n_r <= cap, "more keypoints than the extractor's capacity");
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    const size_t kb = (size_t)cap * sizeof(plp_keypoint), db = (size_t)cap * 32;
-    const size_t o_kl = 0, o_kr = o_kl + kb, o_dl = o_kr + kb, o_dr = o_dl + db, o_n = o_dr + db, o_x = o_n + 16,
-                 o_d = o_x + (size_t)cap * 4, o_b = o_d + (size_t)cap * 4, total = o_b + (size_t)cap * 4;
-    uint8_t *d = nullptr;
-    PLP_TRY(ctx_scratch(ctx, 3, total, (void **)&d));
+    // one frame of the batched layout: keypoints and descriptors in slots of `cap`
+    DevLayout L;
+    const plp_keypoint *d_kl, *d_kr;
+    const uint8_t *d_dl, *d_dr;
+    const int32_t *d_n;
+    float *d_x, *d_depth;
+    int32_t *d_best;
     const int32_t n2[2] = {n_l, n_r};
-    cudaStream_t s = ctx->stream;
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_kl, kp_l, (size_t)n_l * sizeof(plp_keypoint), cudaMemcpyHostToDevice, s));
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_kr, kp_r, (size_t)n_r * sizeof(plp_keypoint), cudaMemcpyHostToDevice, s));
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_dl, desc_l, (size_t)n_l * 32, cudaMemcpyHostToDevice, s));
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_dr, desc_r, (size_t)n_r * 32, cudaMemcpyHostToDevice, s));
-    PLP_CUDA_TRY(cudaMemcpyAsync(d + o_n, n2, 8, cudaMemcpyHostToDevice, s));
-    PLP_TRY(plp_stereo_compute_batch_dev(ctx, left, right, 1, (const plp_keypoint *)(d + o_kl), d + o_dl,
-                                         (const int32_t *)(d + o_n), (const plp_keypoint *)(d + o_kr), d + o_dr,
-                                         (const int32_t *)(d + o_n + 4), focal_x_baseline, true_baseline, (float *)(d + o_x),
-                                         (float *)(d + o_d), (int32_t *)(d + o_b)));
-    PLP_CUDA_TRY(cudaMemcpyAsync(x_right_out, d + o_x, (size_t)n_l * 4, cudaMemcpyDeviceToHost, s));
-    PLP_CUDA_TRY(cudaMemcpyAsync(depths_out, d + o_d, (size_t)n_l * 4, cudaMemcpyDeviceToHost, s));
-    if (best_right_out) PLP_CUDA_TRY(cudaMemcpyAsync(best_right_out, d + o_b, (size_t)n_l * 4, cudaMemcpyDeviceToHost, s));
-    PLP_CUDA_TRY(cudaStreamSynchronize(s));
+    L.in(d_kl, kp_l, n_l, cap);
+    L.in(d_kr, kp_r, n_r, cap);
+    L.in(d_dl, desc_l, (size_t)n_l * 32, (size_t)cap * 32);
+    L.in(d_dr, desc_r, (size_t)n_r * 32, (size_t)cap * 32);
+    L.in(d_n, n2, 2);
+    L.out(d_x, cap);
+    L.out(d_depth, cap);
+    L.out(d_best, cap);
+    PLP_TRY(stage(ctx, 3, L));
+    PLP_TRY(plp_stereo_compute_batch_dev(ctx, left, right, 1, d_kl, d_dl, d_n, d_kr, d_dr, d_n + 1, focal_x_baseline,
+                                         true_baseline, d_x, d_depth, d_best));
+    PLP_CUDA_TRY(to_host(ctx, x_right_out, d_x, n_l));
+    PLP_CUDA_TRY(to_host(ctx, depths_out, d_depth, n_l));
+    if (best_right_out) PLP_CUDA_TRY(to_host(ctx, best_right_out, d_best, n_l));
+    PLP_CUDA_TRY(cudaStreamSynchronize(ctx->stream));
     return PLP_OK;
 }
 

@@ -1,12 +1,18 @@
 // tracker.h -- internal: the state of a plp_tracker, shared by pipeline.cu (motion_based_track) and local_map.cu
 // (optimize_current_frame_with_local_map, which reads what the motion call left on the device).
 #pragma once
+#include <memory>
+
 #include "common.cuh"
 #include "camera_jobs.h"
 #include "match_jobs.h"
 #include "pose_jobs.h"
 
 namespace plp {
+
+namespace lm {
+struct LocalDev;  // local_map_kernels.cuh
+}
 
 struct TrackDev {
     int batch, cap, num_levels;
@@ -68,6 +74,7 @@ struct plp_tracker {
     bool has_motion = false;
     // local-map tracking (plp_tracker_reserve_local_map); d_local == nullptr until reserved
     int max_local = 0;
-    float level_thr[16];             // predict_scale_level thresholds (plp_fuse_level_thresholds)
     uint8_t *d_local = nullptr;      // one allocation, carved by local_map.cu
+    // the job with that scratch bound and the predict_scale_level thresholds set; every call adds its own inputs
+    std::shared_ptr<plp::lm::LocalDev> local;
 };
