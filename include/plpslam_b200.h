@@ -786,6 +786,10 @@ PLP_API plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale
  *   pose_out [batch x 16]; num_tracked_out = inliers of the second pose optimisation (the caller applies 20, or 40
  *     after relocalisation); n_inliers_out = the optimiser's return value; lm_iters_out;
  *   status_out: 0, 1 = the frame's local list exceeds max_local_points, 2 = a last_local_idx entry is out of range.
+ * After a plp_tracker_keyframe_track_batch_dev of the same batch (batch <= its batch), a frame with stage 1 is taken from
+ * that call instead: active iff its keyframe track succeeded, starting from its pose, with the keyframe landmarks its pose
+ * optimisation observed excluded through plp_track_keyframe.local_idx, and matched_out holding keyframe rows; status 2
+ * if its local_idx block is missing or out of range.
  * A frame whose motion track failed, or with status != 0, keeps the motion pose with every per-keypoint output -1, every
  * observable flag 0, 0 iterations and num_tracked 0.  Without a reservation, or with batch > max_batch or no preceding
  * motion track: PLP_ERR_INVALID and nothing is launched. */
@@ -794,6 +798,58 @@ PLP_API plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int bat
                                                          uint8_t *d_observable_out, double *d_pose_out,
                                                          int32_t *d_num_tracked_out, int32_t *d_n_inliers_out,
                                                          int32_t *d_lm_iters_out, int32_t *d_status_out);
+
+/* frame_tracker::bow_match_based_track (module/frame_tracker.cc:126-189) against each frame's reference keyframe
+ * (curr_frm.ref_keyfrm_), for the frames of the tracker's most recent motion_track_batch_dev that the reference hands to
+ * it: the motion model is not usable, or the motion track failed.  frame::compute_bow (transform, levelsup 4) ->
+ * bow_tree::match_frame_and_keyframe (Lowe 0.7, orientation check) -> below 20 matches the frame fails; else
+ * pose_optimizer::optimize from last_frm.cam_pose_cw_ (the motion call's pose_last) -> discard_outliers.  Monocular. */
+typedef struct plp_track_keyframe { /* device pointers except num_keyframes; keyframe k owns rows [row_offsets[k], row_offsets[k+1]) */
+    int32_t num_keyframes;           /* K (host value), at most the reserved max_keyframes                              */
+    const int32_t *kf_of_frame;      /* batch: index of frame b's reference keyframe                                    */
+    const int32_t *row_offsets;      /* K + 1                                                                            */
+    const uint8_t *desc;             /* x 32: descriptors_                                                               */
+    const float *angle;              /* keypts_[i].angle                                                                 */
+    const uint8_t *valid;            /* lm && !lm->will_be_erased(); NULL == all                                         */
+    const double *pos_w;             /* x 3: lm->get_pos_in_world() (read for valid rows only)                           */
+    const int32_t *fv_offsets;       /* K + 1: keyframe k's bow_feat_vec_ nodes are [fv_offsets[k], fv_offsets[k+1])     */
+    const uint32_t *node_ids;        /* ascending within a keyframe                                                      */
+    const int32_t *node_begin;       /* nodes + 1: node a's rows are indices[node_begin[a] .. node_begin[a+1])           */
+    const uint32_t *indices;         /* keyframe-local row numbers                                                       */
+    const int32_t *local_idx;        /* optional: per frame, one entry per row of its keyframe: that landmark's index in
+                                        the frame's local list (plp_track_local), or -1; read by the local-map stage     */
+    const int32_t *local_idx_offsets; /* batch + 1 (with local_idx)                                                      */
+} plp_track_keyframe;
+
+/* Allocates the keyframe-track scratch for max_batch frames whose keyframes hold up to max_keyframe_points rows each, in
+ * tables of up to max_keyframes keyframes; call it once, outside the hot path. */
+PLP_API plp_status plp_tracker_reserve_keyframe_track(plp_tracker *t, int max_keyframes, int max_keyframe_points);
+/* Follows motion_track_batch_dev on the same stream (batch <= that call's batch) and reads its inputs, outputs and
+ * scratch; writes none of them.  Frame b runs the stage iff d_motion_valid[b] == 0 (NULL: all 1; the reference's
+ * velocity_is_valid_ && last_reloc_frm_id_ + 2 < curr_frm_.id_) or its motion num_valid < 20.  No host synchronisation.
+ * vocab must live on the tracker's device; its kernels run on the tracker's stream.  Outputs (device):
+ *   stage_out[batch]: 0 = the motion result stands, 1 = the keyframe stage ran (tracking succeeded iff num_valid >= 20);
+ *   kf_matched_out[batch x kp_capacity]: the keyframe row each keypoint keeps after discard_outliers, or -1;
+ *   num_bow_matches_out[batch]: match_frame_and_keyframe's count (0 where the stage did not run);
+ *   pose_out[batch x 16]: the optimiser result, or pose_last where it did not run;
+ *   num_valid_out, n_inliers_out, lm_iters_out [batch] (0 where the optimiser did not run);
+ *   status_out[batch]: 0, 1 = the keyframe has more than max_keyframe_points rows, 2 = kf_of_frame out of [0, K); such a
+ *     frame (stage 1) fails like a track with no match.
+ * Without a reservation, with K > max_keyframes, with no preceding motion track or with batch above its batch:
+ * PLP_ERR_INVALID and nothing is launched.  A following local_map_track_batch_dev of the same batch starts each stage-1
+ * frame from this call's result (see INTEGRATION.md). */
+PLP_API plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *vocab, int batch,
+                                                        const plp_track_keyframe *kf, const uint8_t *d_motion_valid,
+                                                        int32_t *d_stage_out, int32_t *d_kf_matched_out,
+                                                        int32_t *d_num_bow_matches_out, double *d_pose_out,
+                                                        int32_t *d_num_valid_out, int32_t *d_n_inliers_out,
+                                                        int32_t *d_lm_iters_out, int32_t *d_status_out);
+/* The BoW rows (transform with levelsup 4: word id, node id, weight; max_batch x kp_capacity) of the most recent
+ * keyframe_track_batch_dev, for the frames it ran the stage on (stage 1, status 0): device pointers owned by the
+ * tracker, valid once its stream has reached that call.  A keyframe made from such a frame takes its bow_vec_ /
+ * bow_feat_vec_ from these rows (plp_bow_transform's layout) instead of transforming again. */
+PLP_API plp_status plp_tracker_keyframe_bow(const plp_tracker *t, const int32_t **d_word_id, const int32_t **d_node_id,
+                                            const float **d_weight);
 
 /* ------------------------------------------------------------------------ */
 /* local bundle adjustment (optimize/local_bundle_adjuster*.cc)               */

@@ -37,6 +37,7 @@ FILE_FLAGS = {
     "plane.cu": NO_FMA,
     "camera.cu": NO_FMA,
     "local_map.cu": NO_FMA,
+    "keyframe_track.cu": NO_FMA,
 }
 
 

@@ -667,6 +667,10 @@ class BowVocabulary:
         except Exception:
             pass
 
+    @property
+    def handle(self):
+        return self._h
+
     def info(self):
         v = [C.c_int32() for _ in range(4)]
         self._ctx._check(self._lib.plp_bow_vocab_info(self._h, *[C.byref(x) for x in v]))

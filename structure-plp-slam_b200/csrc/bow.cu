@@ -12,41 +12,22 @@
 // (distance, list position)), one CTA per (side-1, side-2) pair so that the orientation histogram is a block reduction.
 #include "common.cuh"
 #include "bow_kernels.cuh"
+#include "bow_vocab.h"
 
 #include <algorithm>
 #include <map>
 #include <stdio.h>
 
-struct plp_bow_vocab {
-    plp_ctx *ctx = nullptr;
-    int k = 0, L = 0, num_nodes = 0, num_words = 0, max_children = 0;
-    uint8_t *d_desc = nullptr;          // num_nodes x 32
-    uint32_t *d_child_begin = nullptr;  // num_nodes + 1
-    uint32_t *d_children = nullptr;     // num_nodes - 1 node ids, grouped by parent, ascending id inside a group
-    float *d_weight = nullptr;          // num_nodes
-    int32_t *d_word_id = nullptr;       // num_nodes (-1 for inner nodes)
-};
-
 namespace plp {
 
 namespace {
-
-static VocabDev vocab_dev(const plp_bow_vocab *v) {
-    VocabDev V;
-    V.desc = v->d_desc;
-    V.child_begin = v->d_child_begin;
-    V.children = v->d_children;
-    V.weight = v->d_weight;
-    V.word_id = v->d_word_id;
-    return V;
-}
 
 static plp_status launch_transform(plp_bow_vocab *v, const uint8_t *d_desc, int n, int levelsup, int32_t *d_word,
                                    int32_t *d_node, float *d_weight) {
     plp_ctx *ctx = v->ctx;
     const int nid_level = v->L - levelsup;  // <= 0: the root (node id 0)
     const VocabDev V = vocab_dev(v);
-    const int G = v->max_children <= 4 ? 4 : v->max_children <= 8 ? 8 : v->max_children <= 16 ? 16 : 32;
+    const int G = transform_group(v);
     const int groups_per_block = 256 / G;
     const int blocks = div_up(n, groups_per_block);
     switch (G) {

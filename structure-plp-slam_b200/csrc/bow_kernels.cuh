@@ -22,16 +22,17 @@ struct VocabDev {
     const int32_t *word_id;
 };
 
-// TemplatedVocabulary::transform(feature, word_id, weight, &nid, levelsup)
+struct BowWord {
+    int32_t word, node;
+    float weight;
+};
+
+// TemplatedVocabulary::transform(feature, word_id, weight, &nid, levelsup) of one descriptor by a group of G lanes
+// (gl = lane in the group).  Every lane of the warp must take part: the descent's loop condition is a warp vote.
 template <int G>
-__global__ void __launch_bounds__(256) bow_transform_kernel(VocabDev V, const uint8_t *__restrict__ desc, int n,
-                                                            int nid_level, int32_t *__restrict__ word_out,
-                                                            int32_t *__restrict__ node_out, float *__restrict__ weight_out) {
-    const int gid = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) / G);
-    const int gl = (int)(threadIdx.x % G);
-    const int row = min(gid, n - 1);  // surplus groups shadow the last row (shuffles need every lane) and do not store
+__device__ __forceinline__ BowWord bow_descend(const VocabDev &V, const uint8_t *__restrict__ d, int nid_level, int gl) {
     uint4 q0, q1;
-    load_desc(desc + 32 * (size_t)row, q0, q1);
+    load_desc(d, q0, q1);
     int final_id = 0, nid = 0, level = 0;
     uint32_t beg = V.child_begin[0], end = V.child_begin[1];
     const bool empty_vocab = beg == end;
@@ -53,10 +54,25 @@ __global__ void __launch_bounds__(256) bow_transform_kernel(VocabDev V, const ui
             end = V.child_begin[final_id + 1];
         }
     }
+    BowWord w;
+    w.word = empty_vocab ? -1 : V.word_id[final_id];
+    w.node = nid;
+    w.weight = empty_vocab ? 0.0f : V.weight[final_id];
+    return w;
+}
+
+template <int G>
+__global__ void __launch_bounds__(256) bow_transform_kernel(VocabDev V, const uint8_t *__restrict__ desc, int n,
+                                                            int nid_level, int32_t *__restrict__ word_out,
+                                                            int32_t *__restrict__ node_out, float *__restrict__ weight_out) {
+    const int gid = (int)((blockIdx.x * (unsigned)blockDim.x + threadIdx.x) / G);
+    const int gl = (int)(threadIdx.x % G);
+    const int row = min(gid, n - 1);  // surplus groups shadow the last row (shuffles need every lane) and do not store
+    const BowWord w = bow_descend<G>(V, desc + 32 * (size_t)row, nid_level, gl);
     if (gl == 0 && gid < n) {
-        word_out[gid] = empty_vocab ? -1 : V.word_id[final_id];
-        node_out[gid] = nid;
-        weight_out[gid] = empty_vocab ? 0.0f : V.weight[final_id];
+        word_out[gid] = w.word;
+        node_out[gid] = w.node;
+        weight_out[gid] = w.weight;
     }
 }
 

@@ -3,7 +3,7 @@
 //       search_local_landmarks (frame::can_observe + projection::match_frame_and_landmarks, Lowe ratio 0.8)
 //     + pose_optimizer::optimize + the outlier drop and tracked-landmark count
 // for the batch of the tracker's most recent plp_tracker_motion_track_batch_dev, on the same stream and without leaving
-// HBM.  It reads that call's inputs, outputs and scratch (tracker.h) and writes separate outputs, so the motion
+// HBM.  When a plp_tracker_keyframe_track_batch_dev followed that call, its stage-1 frames start from the keyframe track.  It reads that call's inputs, outputs and scratch (tracker.h) and writes separate outputs, so the motion
 // outputs stay as that call wrote them.  Device code: local_map_kernels.cuh.  The window matcher (ratio path) and the
 // pose optimiser are the existing launchers, and the predict_scale_level table is plp_fuse_level_thresholds'.
 //
@@ -97,6 +97,8 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
     PLP_REQUIRE(t->has_motion && batch <= t->motion.batch,
                 "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
+    PLP_REQUIRE(!t->has_kf || batch <= t->kf_batch,
+                "the batch must not exceed that of the plp_tracker_keyframe_track_batch_dev that followed the motion track");
     PLP_REQUIRE(margin > 0.0f, "margin");
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
@@ -116,6 +118,7 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.motion_jobs = M.posejobs;
     D.obs_last = M.obs_last;
     for (int l = 0; l < 16; ++l) D.inv_level_sigma_sq[l] = M.inv_level_sigma_sq[l];
+    if (t->has_kf) D.kf = t->kf_track;  // else D.kf.stage stays null: every frame starts from its motion track
     D.pos_w = local->pos_w;
     D.normal = local->obs_mean_normal;
     D.min_d = local->min_valid_dist;

@@ -17,6 +17,7 @@
 #include "camera_kernels.cuh"
 #include "match_kernels.cuh"
 #include "pose_kernels.cuh"
+#include "track_common.cuh"
 #include "tracker.h"
 
 namespace plp {
@@ -98,55 +99,25 @@ __global__ void track_retry_gate_kernel(TrackDev T) {
 
 // 2D-3D observations of the matched keypoints, in keypoint order (pose_optimizer.cc:126-151)
 __global__ void track_gather_kernel(TrackDev T) {
-    __shared__ int warp_sums[8];
-    __shared__ int s_base;
     const int b = blockIdx.x, tid = threadIdx.x;
-    const int n = T.n_kp[b];
     const size_t base = (size_t)b * T.cap;
     const int l0 = T.last_offsets[b];
     const bool enough = T.num_matches[b] >= (uint32_t)kNumMatchesThr;  // frame_tracker.cc:73-77
-    if (tid == 0) s_base = 0;
-    __syncthreads();
-    for (int start = 0; start < n; start += 256) {
-        const int i = start + tid;
-        int q = -1;
-        if (i < n && enough) q = T.matched[base + i];
-        const int flag = q >= 0;
-        // ordered compaction
-        const unsigned bal = __ballot_sync(0xffffffffu, flag);
-        const int lane = tid & 31, warp = tid >> 5;
-        if (lane == 0) warp_sums[warp] = __popc(bal);
-        __syncthreads();
-        int off = s_base;
-        for (int w = 0; w < warp; ++w) off += warp_sums[w];
-        off += __popc(bal & ((1u << lane) - 1));
-        if (flag) {
-            plp_pt_obs o;
-            const double *X = T.last_pos_w + 3 * (size_t)(l0 + q);
-            o.pos_w[0] = X[0];
-            o.pos_w[1] = X[1];
-            o.pos_w[2] = X[2];
-            o.obs_x = T.x[base + i];
-            o.obs_y = T.y[base + i];
-            o.x_right = -1.0f;
-            o.inv_sigma_sq = T.inv_level_sigma_sq[T.octave[base + i]];
-            T.obs[base + off] = o;
+    const int32_t *matched = T.matched + base;
+    const int n_obs = compact_in_order<256>(
+        T.n_kp[b], [&](int i) { return enough && matched[i] >= 0; },
+        [&](int i, int off) {
+            const int q = matched[i];
+            T.obs[base + off] = point_obs(T.last_pos_w + 3 * (size_t)(l0 + q), T.x[base + i], T.y[base + i],
+                                          T.inv_level_sigma_sq[T.octave[base + i]]);
             T.obs_kp[base + off] = i;
             T.obs_last[base + off] = q;
-        }
-        __syncthreads();
-        if (tid == 0) {
-            int tot = 0;
-            for (int w = 0; w < 8; ++w) tot += warp_sums[w];
-            s_base += tot;
-        }
-        __syncthreads();
-    }
+        });
     if (tid == 0) {
         PoseJob J;
         J.T_in = T.pose_pred + 16 * (size_t)b;
         J.pts = T.obs + base;
-        J.n_pts = s_base;
+        J.n_pts = n_obs;
         J.lines = nullptr;
         J.n_lines = 0;
         J.T_out = T.pose_out + 16 * (size_t)b;
@@ -160,28 +131,12 @@ __global__ void track_gather_kernel(TrackDev T) {
 
 // frame_tracker::discard_outliers (frame_tracker.cc:253-283)
 __global__ void track_finish_kernel(TrackDev T) {
-    __shared__ int s_cnt;
-    const int b = blockIdx.x, tid = threadIdx.x;
+    const int b = blockIdx.x;
     const size_t base = (size_t)b * T.cap;
-    const int n_obs = T.posejobs[b].n_pts;
     const bool enough = T.num_matches[b] >= (uint32_t)kNumMatchesThr;
-    if (tid == 0) s_cnt = 0;
-    __syncthreads();
-    int valid = 0;
-    if (enough) {
-        for (int k = tid; k < n_obs; k += blockDim.x) {
-            if (T.obs_outlier[base + k])
-                T.matched[base + T.obs_kp[base + k]] = -1;
-            else
-                ++valid;
-        }
-    } else {
-        const int n = T.n_kp[b];
-        for (int i = tid; i < n; i += blockDim.x) T.matched[base + i] = -1;
-    }
-    atomicAdd(&s_cnt, valid);
-    __syncthreads();
-    if (tid == 0) T.num_valid[b] = s_cnt;
+    const int valid = discard_outliers<256>(T.n_kp[b], T.posejobs[b].n_pts, enough, T.obs_outlier + base,
+                                            T.obs_kp + base, T.matched + base);
+    if (threadIdx.x == 0) T.num_valid[b] = valid;
 }
 
 }  // namespace
@@ -292,6 +247,7 @@ void plp_tracker_destroy(plp_tracker *t) {
     cudaStreamSynchronize(t->ctx->stream);
     if (t->d_block) cudaFree(t->d_block);
     if (t->d_local) cudaFree(t->d_local);
+    if (t->d_kf) cudaFree(t->d_kf);
     delete t;
 }
 
@@ -308,6 +264,7 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
                 "last-frame arrays");
     plp_ctx *ctx = t->ctx;
     t->has_motion = false;
+    t->has_kf = false;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     TrackDev T = t->dev;
     T.batch = batch;

@@ -1,10 +1,12 @@
-// tracker.h -- internal: the state of a plp_tracker, shared by pipeline.cu (motion_based_track) and local_map.cu
-// (optimize_current_frame_with_local_map, which reads what the motion call left on the device).
+// tracker.h -- internal: the state of a plp_tracker, shared by pipeline.cu (motion_based_track), keyframe_track.cu
+// (bow_match_based_track) and local_map.cu (optimize_current_frame_with_local_map), which read what the motion call
+// left on the device.
 #pragma once
 #include <memory>
 
 #include "common.cuh"
 #include "camera_jobs.h"
+#include "keyframe_track.h"
 #include "match_jobs.h"
 #include "pose_jobs.h"
 
@@ -12,6 +14,9 @@ namespace plp {
 
 namespace lm {
 struct LocalDev;  // local_map_kernels.cuh
+}
+namespace kt {
+struct KfDev;  // keyframe_track_kernels.cuh
 }
 
 struct TrackDev {
@@ -77,4 +82,12 @@ struct plp_tracker {
     uint8_t *d_local = nullptr;      // one allocation, carved by local_map.cu
     // the job with that scratch bound and the predict_scale_level thresholds set; every call adds its own inputs
     std::shared_ptr<plp::lm::LocalDev> local;
+    // keyframe tracking (plp_tracker_reserve_keyframe_track); d_kf == nullptr until reserved
+    int max_keyframes = 0, max_kf_points = 0;
+    uint8_t *d_kf = nullptr;         // one allocation, carved by keyframe_track.cu
+    std::shared_ptr<plp::kt::KfDev> kf;
+    // the keyframe_track_batch_dev that followed the most recent motion track, for the local-map stage
+    plp::KeyframeTrack kf_track;
+    int kf_batch = 0;
+    bool has_kf = false;
 };

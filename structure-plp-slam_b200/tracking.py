@@ -1,8 +1,9 @@
-"""Device-resident batched front-end: ORB extraction + motion-based tracking (+ optionally the local-map stage) without
-leaving HBM.
+"""Device-resident batched front-end: ORB extraction + motion-based tracking (+ optionally the keyframe tracker and the
+local-map stage) without leaving HBM.
 
 Thin ctypes layer over plp_orb_extract_batch_dev + plp_tracker_motion_track_batch_dev (+
-plp_tracker_local_map_track_batch_dev); used by bench.py and the pipeline parity tests.  No compute here.
+plp_tracker_keyframe_track_batch_dev, plp_tracker_local_map_track_batch_dev); used by bench.py and the pipeline parity
+tests.  No compute here.
 """
 from __future__ import annotations
 
@@ -22,6 +23,12 @@ class TrackLast(C.Structure):
 class TrackLocal(C.Structure):
     _fields_ = [("pos_w", _P), ("obs_mean_normal", _P), ("min_valid_dist", _P), ("max_valid_dist", _P),
                 ("max_valid_dist_raw", _P), ("desc", _P), ("valid", _P), ("offsets", _P), ("last_local_idx", _P)]
+
+
+class TrackKeyframe(C.Structure):
+    _fields_ = [("num_keyframes", C.c_int32), ("kf_of_frame", _P), ("row_offsets", _P), ("desc", _P), ("angle", _P),
+                ("valid", _P), ("pos_w", _P), ("fv_offsets", _P), ("node_ids", _P), ("node_begin", _P), ("indices", _P),
+                ("local_idx", _P), ("local_idx_offsets", _P)]
 
 
 def _logf(x: float) -> float:
@@ -152,6 +159,9 @@ class FrontEnd:
         self._local_bufs = []
         self._local = None
         self._local_out = None
+        self._kf_bufs = []
+        self._kf = None
+        self._kf_out = None
         self._last_bufs = []
         self._last = None
         self._last_pinned = []   # host copies of the last-frame arrays (end-to-end path: uploaded every step)
@@ -160,9 +170,10 @@ class FrontEnd:
         self._out_layout = None
 
     def close(self):
-        for b in self._local_bufs:
+        for b in self._local_bufs + self._kf_bufs:
             b.free()
         self._local_bufs = []
+        self._kf_bufs = []
         if self._trk is not None:
             self.lib.plp_tracker_destroy(self._trk)
             self._trk = None
@@ -228,6 +239,54 @@ class FrontEnd:
         self._local_offsets = offs
         self._d_observable = DeviceBuffer(self.ctx, max(int(offs[-1]), 1))
         self._local_bufs.append(self._d_observable)
+
+    def reserve_keyframe_track(self, max_keyframes: int, max_keyframe_points: int):
+        """Scratch for keyframe tables of up to max_keyframes keyframes of up to max_keyframe_points rows (outside the
+        hot path), and the outputs of track_keyframe."""
+        self.ctx._check(self.lib.plp_tracker_reserve_keyframe_track(self._trk, C.c_int(max_keyframes),
+                                                                    C.c_int(max_keyframe_points)))
+        B = self.max_batch
+        if self._kf_out is None:
+            self._kf_out = dict(stage=DeviceBuffer(self.ctx, B * 4), matched=DeviceBuffer(self.ctx, B * self.cap * 4),
+                                num_bow=DeviceBuffer(self.ctx, B * 4), pose=DeviceBuffer(self.ctx, B * 128),
+                                num_valid=DeviceBuffer(self.ctx, B * 4), n_inliers=DeviceBuffer(self.ctx, B * 4),
+                                lm_iters=DeviceBuffer(self.ctx, B * 4), status=DeviceBuffer(self.ctx, B * 4),
+                                motion_valid=DeviceBuffer(self.ctx, B))
+
+    def set_keyframes(self, keyframes, kf_of_frame, local_idx=None):
+        """keyframes[k]: dict(desc[n,32], angle[n] (keypts_[i].angle), valid[n]|None (lm && !will_be_erased()),
+        pos_w[n,3], fv=(node_ids, offsets, indices) (bow_feat_vec_ flattened, as capi.fold_bow returns it));
+        kf_of_frame[b]: frame b's reference keyframe.  local_idx (optional, for track_local_map after track_keyframe):
+        per frame, one entry per row of its keyframe -- that landmark's index in the frame's local list, or -1."""
+        for b in self._kf_bufs:
+            b.free()
+        rows = np.zeros(len(keyframes) + 1, np.int32)
+        rows[1:] = np.cumsum([len(k["desc"]) for k in keyframes])
+        fv_offs = np.zeros(len(keyframes) + 1, np.int32)
+        fv_offs[1:] = np.cumsum([len(k["fv"][0]) for k in keyframes])
+        node_begin, base = [], 0
+        for k in keyframes:
+            node_begin.append(np.asarray(k["fv"][1][:-1], np.int64) + base)
+            base += len(k["fv"][2])
+        node_begin = np.concatenate(node_begin + [np.array([base])]).astype(np.int32)
+
+        def cat(key, dt, shape):
+            parts = [np.asarray(k[key], dt).reshape((-1,) + shape) for k in keyframes]
+            return np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0,) + shape, dt))
+        valid = np.ascontiguousarray(np.concatenate(
+            [np.asarray(k["valid"], np.uint8) if k.get("valid") is not None else np.ones(len(k["desc"]), np.uint8)
+             for k in keyframes]))
+        fv = lambda i, dt: np.ascontiguousarray(np.concatenate([np.asarray(k["fv"][i], dt) for k in keyframes]))
+        arrays = [np.ascontiguousarray(kf_of_frame, np.int32), rows, cat("desc", np.uint8, (32,)),
+                  cat("angle", np.float32, ()), valid, cat("pos_w", np.float64, (3,)), fv_offs, fv(0, np.uint32),
+                  node_begin, fv(2, np.uint32)]
+        if local_idx is not None:
+            lio = np.zeros(len(local_idx) + 1, np.int32)
+            lio[1:] = np.cumsum([len(x) for x in local_idx])
+            arrays += [np.ascontiguousarray(np.concatenate([np.asarray(x, np.int32) for x in local_idx])), lio]
+        self._kf_bufs = [DeviceBuffer.from_array(self.ctx, a) for a in arrays]
+        ptrs = [b.ptr for b in self._kf_bufs] + [None] * (12 - len(self._kf_bufs))
+        self._kf = TrackKeyframe(len(keyframes), *ptrs)
 
     # -- end-to-end path: every input of a step comes from pinned host memory, every result goes back ----
     def stage_host_io(self, imgs: np.ndarray):
@@ -319,6 +378,25 @@ class FrontEnd:
             self._d_observable.ptr, o["pose"].ptr, o["num_tracked"].ptr, o["n_inliers"].ptr, o["lm_iters"].ptr,
             o["status"].ptr))
 
+    def track_keyframe(self, batch: int, vocab, motion_valid=None):
+        """bow_match_based_track for the frames of the preceding track() whose motion model is not usable
+        (motion_valid[b] == 0; None: all usable) or whose motion track failed (tracking stream)."""
+        o = self._kf_out
+        if o is None or self._kf is None:
+            raise PlpError("track_keyframe needs reserve_keyframe_track() and set_keyframes() first")
+        mv = None
+        if motion_valid is not None:  # on the tracking stream: an earlier call there may still read the buffer
+            flags = np.ascontiguousarray(motion_valid, np.uint8)
+            assert flags.nbytes <= o["motion_valid"].nbytes
+            tc = self.track_ctx
+            tc._check(self.lib.plp_dev_upload(tc.handle, o["motion_valid"].ptr, flags.ctypes.data_as(_P),
+                                              C.c_size_t(flags.nbytes)))
+            mv = o["motion_valid"].ptr
+        self.ctx._check(self.lib.plp_tracker_keyframe_track_batch_dev(
+            self._trk, vocab.handle, C.c_int(batch), C.byref(self._kf), mv, o["stage"].ptr, o["matched"].ptr,
+            o["num_bow"].ptr, o["pose"].ptr, o["num_valid"].ptr, o["n_inliers"].ptr, o["lm_iters"].ptr,
+            o["status"].ptr))
+
     # -- results --------------------------------------------------------------------------------------
     def _after_tracking(self):
         """The downloads below run on the extraction stream; the tracking outputs are written on the tracking stream."""
@@ -366,6 +444,31 @@ class FrontEnd:
                     n_inliers=o["n_inliers"].download(np.int32, (batch,)),
                     lm_iters=o["lm_iters"].download(np.int32, (batch,)),
                     status=o["status"].download(np.int32, (batch,)))
+
+    def download_keyframe_tracking(self, batch: int):
+        """Results of track_keyframe: per frame the stage flag, the keyframe row kept on each keypoint, the BoW match
+        count, pose, num_valid, n_inliers, LM iterations, status, and the BoW rows (word id, node id, weight per
+        keypoint; meaningful for the frames that ran the stage)."""
+        self._after_tracking()
+        n = self.d_n.download(np.int32, (batch,))
+        o = self._kf_out
+        matched = o["matched"].download(np.int32, (self.max_batch, self.cap))[:batch]
+        w, nd, wt = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        self.ctx._check(self.lib.plp_tracker_keyframe_bow(self._trk, C.byref(w), C.byref(nd), C.byref(wt)))
+        bow = []
+        for p, dt in ((w, np.int32), (nd, np.int32), (wt, np.float32)):
+            a = np.zeros((self.max_batch, self.cap), dt)
+            self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, a.ctypes.data_as(_P), p, C.c_size_t(a.nbytes)))
+            bow.append(a)
+        return dict(stage=o["stage"].download(np.int32, (batch,)),
+                    matched=[matched[b, :n[b]].copy() for b in range(batch)],
+                    num_bow_matches=o["num_bow"].download(np.int32, (batch,)),
+                    pose=o["pose"].download(np.float64, (batch, 4, 4)),
+                    num_valid=o["num_valid"].download(np.int32, (batch,)),
+                    n_inliers=o["n_inliers"].download(np.int32, (batch,)),
+                    lm_iters=o["lm_iters"].download(np.int32, (batch,)),
+                    status=o["status"].download(np.int32, (batch,)),
+                    bow=[tuple(a[b, :n[b]].copy() for a in bow) for b in range(batch)])
 
     def download_tracking(self, batch: int):
         self._after_tracking()
