@@ -922,6 +922,15 @@ PLP_API plp_status plp_ba_solve(plp_ba *ba, volatile const uint8_t *force_stop, 
 PLP_API void plp_ba_destroy(plp_ba *ba);
 /* benchmark hook: run `tries` LM tries (linearise + Schur + solve + update + accept/reject) from the initial state */
 PLP_API plp_status plp_ba_bench_tries(plp_ba *ba, int tries, int32_t *iters_done, int32_t *tries_done);
+/* test read-back of ONE try's linear algebra: from the initial state (Huber kernel on) the lambda-initialisation try and the
+ * first real try run exactly as in plp_ba_bench_tries(ba, 1, ...); then the reduced camera system that try solved comes back:
+ *   packed  n_pairs * 36 + 12 * n_free + 1 doubles, n_pairs = n_free (n_free + 1) / 2:
+ *           [S: the upper 6 x 6 blocks (i, j), i <= j, row-wise over the free keyframes, lambda NOT yet on the diagonal |
+ *            g: 6 n_free | bp = -Jp^T w e: 6 n_free | robust chi2 of the linearisation point]
+ *   dp      6 * n_free: the pose step, solution of (S + lambda I) dp = g (zero if the system was not positive definite)
+ *   lambda  the damping of that try (already inside the Schur term: S = Hpp - sum_l W (Hll + lambda I)^-1 W^T)
+ * Both representations (shared-memory and dense-in-HBM) fill the same layout.  Any of the three outputs may be NULL. */
+PLP_API plp_status plp_ba_debug_try(plp_ba *ba, double *packed, double *dp, double *lambda);
 
 /* multi-GPU: rank 0 creates a 128-byte id, the launcher broadcasts it, every rank joins */
 PLP_API plp_status plp_ba_comm_unique_id(uint8_t id_out[128]);

@@ -102,6 +102,15 @@ class LocalBA:
         self._ctx._check(self._lib.plp_ba_bench_tries(self._h, C.c_int(tries), C.byref(it), C.byref(tr)))
         return it.value, tr.value
 
+    def debug_try(self, n_free: int):
+        """plp_ba_debug_try: (S upper blocks [n_pairs, 6, 6], g, bp, chi2, dp, lambda) of the first real LM try."""
+        n_pairs = n_free * (n_free + 1) // 2
+        packed, dp, lam = np.zeros(n_pairs * 36 + 12 * n_free + 1), np.zeros(6 * n_free), C.c_double(0.0)
+        self._ctx._check(self._lib.plp_ba_debug_try(self._h, packed.ctypes.data_as(_P), dp.ctypes.data_as(_P), C.byref(lam)))
+        nS = n_pairs * 36
+        return dict(S=packed[:nS].reshape(n_pairs, 6, 6), g=packed[nS:nS + 6 * n_free],
+                    bp=packed[nS + 6 * n_free:nS + 12 * n_free], chi2=float(packed[-1]), dp=dp, lam=lam.value, packed=packed)
+
     def close(self):
         if self._h is not None:
             self._lib.plp_ba_destroy(self._h)

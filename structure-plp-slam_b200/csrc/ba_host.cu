@@ -403,13 +403,10 @@ static plp_status ba_solve_impl(plp_ba *b, volatile const uint8_t *force_stop, p
     return PLP_OK;
 }
 
-/* LM tries only (no download): `tries` tries of the first optimize() phase on the current state.  Used by the
- * throughput benchmark (LM iterations per second) -- each try is one full linearise + Schur + solve + update. */
-plp_status plp_ba_bench_tries(plp_ba *b, int tries, int32_t *iters_done, int32_t *tries_done) {
-    PLP_REQUIRE(b && tries >= 1, "args");
+// reset to the initial state, then the lambda-initialisation try and `tries` tries of the first optimize() phase (Huber on)
+static plp_status tries_from_initial_state(plp_ba *b, int tries) {
     plp_ctx *ctx = b->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    BaCollective *coll = b->comm ? ba_comm_collective(b->comm) : nullptr;
     const BaDev &D = b->dev;
     PLP_TRY(ba_launch_init_poses(ctx, D, b->d_T_in));
     if (b->n_pts) PLP_CUDA_TRY(cudaMemcpyAsync(D.pts[0], b->d_pts_in, (size_t)b->n_pts * 24, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -418,12 +415,35 @@ plp_status plp_ba_bench_tries(plp_ba *b, int tries, int32_t *iters_done, int32_t
     if (b->n_pe) PLP_CUDA_TRY(cudaMemsetAsync(D.pt_level, 0, b->n_pe, ctx->stream));
     if (b->n_le) PLP_CUDA_TRY(cudaMemsetAsync(D.ln_level, 0, b->n_le, ctx->stream));
     PLP_TRY(ba_launch_set_state(ctx, D, 1 << 28, 1, 1));
-    (void)coll;
     for (int t = 0; t < tries + 1; ++t) PLP_TRY(launch_try(b));  // +1: the lambda-init try
-    PLP_TRY(ba_launch_decide(ctx, D));
+    return PLP_OK;
+}
+
+/* LM tries only (no download).  Used by the throughput benchmark (LM iterations per second) -- each try is one full
+ * linearise + Schur + solve + update. */
+plp_status plp_ba_bench_tries(plp_ba *b, int tries, int32_t *iters_done, int32_t *tries_done) {
+    PLP_REQUIRE(b && tries >= 1, "args");
+    PLP_TRY(tries_from_initial_state(b, tries));
+    PLP_TRY(ba_launch_decide(b->ctx, b->dev));
     PLP_TRY(read_state(b));
     if (iters_done) *iters_done = b->h_state->it;
     if (tries_done) *tries_done = b->h_state->tries;
+    return PLP_OK;
+}
+
+/* Test read-back: the reduced camera system, the step and the damping of the first real try (see the header).  The state
+ * is read BEFORE the accept / reject decision of that try, which would rescale lambda; the next solve resets the state. */
+plp_status plp_ba_debug_try(plp_ba *b, double *packed, double *dp, double *lambda) {
+    PLP_REQUIRE(b, "null pointer");
+    PLP_TRY(tries_from_initial_state(b, 1));
+    plp_ctx *ctx = b->ctx;
+    const BaDev &D = b->dev;
+    if (packed)
+        PLP_CUDA_TRY(cudaMemcpyAsync(packed, D.packed, ((size_t)D.n_pairs * 36 + 12 * (size_t)D.n_free + 1) * sizeof(double),
+                                     cudaMemcpyDeviceToHost, ctx->stream));
+    if (dp) PLP_CUDA_TRY(cudaMemcpyAsync(dp, D.dp, (size_t)6 * D.n_free * sizeof(double), cudaMemcpyDeviceToHost, ctx->stream));
+    PLP_TRY(read_state(b));
+    if (lambda) *lambda = b->h_state->lambda;
     return PLP_OK;
 }
 

@@ -237,3 +237,148 @@ def make_ba_problem(seed, n_local=20, n_fixed=10, n_points=4000, n_lines=800, n_
                      pt_edge_obs=obs, pt_edge_inv_sigma_sq=isig[octv], plane_edge_lm=pl_lm,
                      plane_edge_fn=planes[plane_of[pl_lm]] if len(pl_lm) else np.zeros((0, 4)),
                      gt=dict(poses=poses_gt, points=X, line_endpoints=line_endpoints), **line_kw)
+
+
+def make_ba_shape_problem(seed, n_free, n_fixed, points, lines=(), stereo_frac=0.0, global_ba=False, empty_free=(),
+                          outlier_free=(), outlier_frac=0.02, pose_sigma=(0.01, 0.03), point_sigma=0.05):
+    """A problem whose OBSERVATION STRUCTURE is prescribed (make_ba_problem draws k ~ U{3..9} observers uniformly, so it never
+    makes a long track, a landmark without a free observer or a keyframe without edges).  Same camera arc, cloud, noise model
+    and field layout as make_ba_problem.
+
+    points / lines: groups of landmarks, in landmark order, each a dict
+        n      landmarks in the group
+        k      observations per landmark: an int, "all" (every keyframe of the pool) or (lo, hi) for U{lo..hi}
+        who    pool the observers are drawn from: "any" keyframe, "free", "fixed", or "one_free" (exactly one free observer,
+               the other k - 1 fixed)
+        plane  (points) True: every point of the group lies on one of the 3 planes and gets a plane edge
+    global_ba: keyframe 0 is the only fixed one (n_fixed is ignored), as optimize::global_bundle_adjuster sets it up;
+        otherwise keyframes [0, n_free) are free and [n_free, n_free + n_fixed) fixed.
+    empty_free: keyframe indices left out of every pool (free keyframes without a single edge).
+    outlier_free: keyframe indices whose every observation (both end points of a line) is displaced by 100..200 px.
+    stereo_frac: fraction of the point edges that carry a right-image coordinate (0: monocular problem).
+
+    The cloud (z in 4..8 m) is in front of every camera of the arc by more than 3 m, so no edge is ever dropped; the degrees
+    that came out are checked against the request and returned as prob.shape = dict(pt_deg, pt_free_deg, ln_deg,
+    ln_free_deg, kf_deg)."""
+    rng = np.random.default_rng(seed)
+    n_kf = n_free + 1 if global_ba else n_free + n_fixed
+    sf, isig = synth.scale_factors(), synth.inv_level_sigma_sq()
+    fixed = np.zeros(n_kf, np.uint8)
+    if global_ba:
+        fixed[0] = 1
+    else:
+        fixed[n_free:] = 1
+    ang = np.linspace(-0.33, 0.33, n_kf)[rng.permutation(n_kf)]
+    poses_gt = np.zeros((n_kf, 4, 4))
+    for i, a in enumerate(ang):
+        c = np.array([6.0 * np.sin(a), 0.15 * np.cos(3 * a), 6.0 - 6.0 * np.cos(a)])
+        zc = np.array([0.0, 0.0, 6.0]) - c
+        zc /= np.linalg.norm(zc)
+        xc = np.cross([0.0, 1.0, 0.0], zc)
+        xc /= np.linalg.norm(xc)
+        R = np.stack([xc, np.cross(zc, xc), zc])
+        poses_gt[i, :3, :3], poses_gt[i, :3, 3], poses_gt[i, 3, 3] = R, -R @ c, 1.0
+    usable = np.ones(n_kf, bool)
+    usable[list(empty_free)] = False
+    pools = dict(any=np.nonzero(usable)[0], free=np.nonzero(usable & (fixed == 0))[0], fixed=np.nonzero(usable & (fixed == 1))[0])
+
+    def observe(groups):
+        kfs, lms, want, l = [], [], [], 0
+        for g in groups:
+            who = g.get("who", "any")
+            for _ in range(g["n"]):
+                pool = pools["fixed" if who == "one_free" else who]
+                k = g["k"]
+                if k == "all":
+                    k = len(pool) + (who == "one_free")
+                elif isinstance(k, tuple):  # like make_ba_problem: a small window caps the draw
+                    k = min(int(rng.integers(k[0], k[1] + 1)), len(pool))
+                if who == "one_free":
+                    ks = np.concatenate([rng.choice(pools["free"], 1), rng.choice(pool, k - 1, replace=False)])
+                else:
+                    ks = rng.choice(pool, k, replace=False)
+                kfs.append(rng.permutation(ks))  # the C ABI groups edges by landmark only: free and fixed observers mix
+                lms.append(np.full(k, l))
+                want.append(k)
+                l += 1
+        cat = lambda x: np.concatenate(x).astype(np.int32) if x else np.zeros(0, np.int32)
+        return cat(kfs), cat(lms), np.array(want, int)
+
+    def in_camera(ekf, Xw):
+        Xc = np.einsum("eij,ej->ei", poses_gt[ekf, :3, :3], Xw) + poses_gt[ekf, :3, 3]
+        assert (Xc[:, 2] > 0.5).all(), "a landmark is behind (or too close to) a camera of the arc"
+        return Xc
+
+    def project(Xc):
+        return np.stack([synth.FX * Xc[:, 0] / Xc[:, 2] + synth.CX, synth.FY * Xc[:, 1] / Xc[:, 2] + synth.CY], 1)
+
+    def displaced(n):  # gross outliers: 100..200 px in a random direction
+        th, r = rng.uniform(0, 2 * np.pi, n), rng.uniform(100, 200, n)
+        return np.stack([r * np.cos(th), r * np.sin(th)], 1)
+
+    bad_kf = np.zeros(n_kf, bool)
+    bad_kf[list(outlier_free)] = True
+    # ---- points
+    n_points = sum(g["n"] for g in points)
+    planes = np.array([[0, 0, 1.0, -7.5], [1.0, 0, 0, -3.0], [0, 1.0, 0, -1.5]])
+    X = np.stack([rng.uniform(-3, 3, n_points), rng.uniform(-2, 2, n_points), rng.uniform(4, 8, n_points)], 1)
+    plane_of = np.full(n_points, -1)
+    l = 0
+    for g in points:
+        if g.get("plane"):
+            plane_of[l:l + g["n"]] = rng.integers(0, 3, g["n"])
+        l += g["n"]
+    for pi in range(3):
+        X[plane_of == pi, int(np.argmax(np.abs(planes[pi, :3])))] = -planes[pi, 3]
+    ekf, elm, pt_want = observe(points)
+    Xc = in_camera(ekf, X[elm])
+    octv = rng.choice(8, len(ekf), p=np.array([217, 181, 151, 126, 105, 87, 73, 60]) / 1000.0)
+    uv = project(Xc) + rng.normal(0, 1, (len(ekf), 2)) * sf[octv][:, None]
+    out = rng.random(len(ekf)) < outlier_frac
+    uv[out] += rng.normal(0, 30, (out.sum(), 2))
+    uv[bad_kf[ekf]] += displaced(int(bad_kf[ekf].sum()))
+    xr = np.full(len(ekf), -1.0)
+    if stereo_frac > 0:
+        has = rng.random(len(ekf)) < stereo_frac
+        xr[has] = (uv[:, 0] - synth.BF / Xc[:, 2] + rng.normal(0, 1, len(ekf)) * sf[octv])[has]
+    obs = np.concatenate([uv, xr[:, None]], 1).astype(np.float32)
+    # ---- lines
+    n_lines = sum(g["n"] for g in lines)
+    line_kw, line_endpoints, lkf, llm, ln_want = {}, np.zeros((0, 6)), np.zeros(0, np.int32), np.zeros(0, np.int32), np.zeros(0, int)
+    if n_lines:
+        P = np.stack([rng.uniform(-3, 3, n_lines), rng.uniform(-2, 2, n_lines), rng.uniform(4.5, 7.5, n_lines)], 1)
+        d = rng.normal(0, 1, (n_lines, 3))
+        d /= np.linalg.norm(d, axis=1, keepdims=True)
+        Q = P + d * rng.uniform(0.5, 2.0, (n_lines, 1))
+        lkf, llm, ln_want = observe(lines)
+        lobs = np.concatenate([project(in_camera(lkf, P[llm])), project(in_camera(lkf, Q[llm]))], 1)
+        lobs += rng.normal(0, 1, lobs.shape)
+        lout = rng.random(len(lkf)) < outlier_frac
+        lobs[lout, :2] += rng.normal(0, 30, (lout.sum(), 2))
+        lobs[bad_kf[lkf]] += np.concatenate([displaced(int(bad_kf[lkf].sum())), displaced(int(bad_kf[lkf].sum()))], 1)
+        Pn, Qn = P + rng.normal(0, point_sigma, P.shape), Q + rng.normal(0, point_sigma, Q.shape)
+        line_endpoints = np.concatenate([Pn, Qn], 1)
+        line_kw = dict(line_plucker=synth.plucker_from_endpoints(Pn, Qn), line_edge_kf=lkf, line_edge_lm=llm,
+                       line_edge_obs=lobs.astype(np.float32), line_edge_inv_sigma_sq=np.ones(len(lkf), np.float32))
+    # ---- perturbed free poses and landmarks
+    poses = poses_gt.copy()
+    for k in np.nonzero(fixed == 0)[0]:
+        xi = np.concatenate([rng.normal(0, pose_sigma[0], 3), rng.normal(0, pose_sigma[1], 3)])
+        dT = np.eye(4)
+        dT[:3, :3], dT[:3, 3] = synth.so3_exp(xi[:3]), xi[3:]
+        poses[k] = dT @ poses[k]
+    pl_lm = np.nonzero(plane_of >= 0)[0].astype(np.int32)
+    prob = BAProblem(stereo=stereo_frac > 0, kf_pose_cw=poses, kf_fixed=fixed, pt_pos_w=X + rng.normal(0, point_sigma, X.shape),
+                     pt_edge_kf=ekf, pt_edge_lm=elm, pt_edge_obs=obs, pt_edge_inv_sigma_sq=isig[octv], plane_edge_lm=pl_lm,
+                     plane_edge_fn=planes[plane_of[pl_lm]] if len(pl_lm) else np.zeros((0, 4)),
+                     gt=dict(poses=poses_gt, points=X, line_endpoints=line_endpoints), **line_kw)
+    # ---- the shape that came out is the shape that was asked for
+    free_e, free_l = (fixed[prob.pt_edge_kf] == 0).astype(float), (fixed[prob.line_edge_kf] == 0).astype(float)
+    prob.shape = dict(pt_deg=np.bincount(prob.pt_edge_lm, minlength=n_points),
+                      pt_free_deg=np.bincount(prob.pt_edge_lm, weights=free_e, minlength=n_points).astype(int),
+                      ln_deg=np.bincount(prob.line_edge_lm, minlength=n_lines),
+                      ln_free_deg=np.bincount(prob.line_edge_lm, weights=free_l, minlength=n_lines).astype(int),
+                      kf_deg=np.bincount(np.concatenate([prob.pt_edge_kf, prob.line_edge_kf]), minlength=n_kf))
+    assert np.array_equal(prob.shape["pt_deg"], pt_want) and np.array_equal(prob.shape["ln_deg"], ln_want)
+    assert (prob.shape["kf_deg"][list(empty_free)] == 0).all()
+    return prob

@@ -25,7 +25,17 @@ size_t solve_smem(int n_free) {
     return (n * (n + 1) / 2 + 2 * n + 21 * (size_t)n_free) * 8 + 64;
 }
 unsigned div_up_u(size_t a, size_t b) { return (unsigned)((a + b - 1) / b); }
+// read-back of the first real try of the next emu_ba_solve (what plp_ba_debug_try downloads on the GPU)
+double *g_cap_packed = nullptr, *g_cap_dp = nullptr, *g_cap_lambda = nullptr;
 }  // namespace
+
+// The next emu_ba_solve copies out, after its second try (the first after the lambda initialisation) and before that try's
+// accept / reject decision: packed [S upper blocks | g | bp | chi2] (n_pairs * 36 + 12 n_free + 1), dp (6 n_free), lambda.
+extern "C" void emu_ba_capture_try(double *packed, double *dp, double *lambda) {
+    g_cap_packed = packed;
+    g_cap_dp = dp;
+    g_cap_lambda = lambda;
+}
 
 // mode 0: local BA (optimize(first) with Huber, classification, optimize(second) without, classification);
 // mode 1 / 2: one optimize(first) with / without the Huber kernel (global BA).  num_ctas: landmark shards (CTAs) to emulate.
@@ -168,6 +178,7 @@ extern "C" int emu_ba_solve(double fx, double fy, double cx, double cy, double b
 
     const size_t lin_smem = linearize_smem(n_free, n_pairs, pool_cap), sol_smem = solve_smem(n_free);
     const unsigned decide_threads = (unsigned)std::max(64, std::min(512, (n_kf * 12 + 31) / 32 * 32));
+    int tries_launched = 0;
     auto launch_try = [&]() {
         if (getenv("EMU_BA_TRACE")) fprintf(stderr, "[emu ba] try: phase %d it %d tries %d lambda %g chi %g\n", state.phase, state.it, state.tries, state.lambda, state.current_chi);
         emu_launch2(ba_decide_kernel, 1u, 1u, decide_threads, (size_t)0, D);
@@ -179,6 +190,12 @@ extern "C" int emu_ba_solve(double fx, double fy, double cx, double cy, double b
         emu_launch2(ba_solve_kernel, 1u, 1u, (unsigned)kSolveThreads, sol_smem, D);
         if (getenv("EMU_BA_TRACE")) fprintf(stderr, "  update\n");
         emu_launch2(ba_update_kernel, (unsigned)G, 1u, (unsigned)kBaThreads, (size_t)6 * n_free * sizeof(double), D);
+        if (++tries_launched == 2 && g_cap_packed) {
+            memcpy(g_cap_packed, packed.data(), (size_t)packed_sum_len * sizeof(double));
+            memcpy(g_cap_dp, dp.data(), (size_t)6 * n_free * sizeof(double));
+            *g_cap_lambda = state.lambda;
+            g_cap_packed = nullptr;
+        }
     };
     auto run_optimize = [&](int n, int robust, bool first) {  // ba_host.cu run_optimize
         emu_launch2(ba_set_state_kernel, 1u, 1u, 1u, (size_t)0, D, n, robust, first ? 1 : 0);

@@ -202,6 +202,34 @@ def test_local_ba_points_lines_planes_matches_full_system_lm(orc, seed):
     _compare(o, g, it1, it2, pt_out, ln_out, prob, tol=1e-5, trace=trace, rho_tol=5e-2, lam_tol=1e-2)
 
 
+def test_local_ba_with_an_edgeless_keyframe_and_fixed_only_landmarks_matches_full_system_lm(orc):
+    """Shapes make_ba_problem cannot draw: a free keyframe without a single edge (zero Hpp block: g2o leaves such a vertex
+    out of the active set, here its step is 0 / lambda = 0), landmarks seen by fixed keyframes only, landmarks with two observations, points with 33 edges.  The oracle accepts them
+    and walks the path of the full-system restatement."""
+    prob = ba_data.make_ba_shape_problem(
+        9, 5, 34, empty_free=(4,), outlier_frac=0.05,
+        points=[dict(n=3, k=33), dict(n=6, k=4, who="fixed"), dict(n=8, k=2), dict(n=4, k=5, who="one_free"), dict(n=100, k=(3, 9))])
+    assert prob.shape["kf_deg"][4] == 0 and (prob.shape["pt_free_deg"][3:9] == 0).all() and (prob.shape["pt_deg"][:3] == 33).all()
+    o = ba_data.oracle_local_ba(orc, prob)
+    trace = _oracle_trace(orc)
+    assert np.allclose(o.kf_pose_cw.reshape(-1, 4, 4)[4], prob.kf_pose_cw[4], atol=1e-12)
+    g = bn.Graph(prob, CAM)
+    it1, it2, pt_out, ln_out = g.local_ba()
+    _compare(o, g, it1, it2, pt_out, ln_out, prob, trace=trace)
+
+
+def test_make_ba_problem_is_unchanged_by_the_shape_generator():
+    """The problems the GPU parity tests and the benchmark were tuned on: one checksum over every field of one seed."""
+    import hashlib
+    prob = ba_data.make_ba_problem(42, n_local=6, n_fixed=3, n_points=200, n_lines=40, n_plane_pts=10, stereo=True)
+    h = hashlib.sha256()
+    for a in (prob.kf_pose_cw, prob.kf_fixed, prob.pt_pos_w, prob.pt_edge_kf, prob.pt_edge_lm, prob.pt_edge_obs,
+              prob.pt_edge_inv_sigma_sq, prob.line_plucker, prob.line_edge_kf, prob.line_edge_lm, prob.line_edge_obs,
+              prob.plane_edge_lm, prob.plane_edge_fn):
+        h.update(np.ascontiguousarray(a).tobytes())
+    assert h.hexdigest() == "fc4a0df26339f4dfd9333398fd24f86ba771e17dd16b5ece1e033f5a63fe542b"
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # (iii) the optimum equals scipy's for the same cost
 # ---------------------------------------------------------------------------------------------------------------------

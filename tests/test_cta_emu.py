@@ -583,15 +583,73 @@ def _emu_ba_solve(emu, prob, first=5, second=10, mode=0, ctas=3):
     return kf, pts[:n_pts], ln[:n_l], po[:len(prob.pt_edge_kf)], lo[:len(prob.line_edge_kf)], tuple(int(v) for v in it)
 
 
-def test_local_ba_kernels_equal_oracle(ba_emu):
+def _ba_long_tracks(seed, n_free, n_fixed, lines=True, **kw):
+    """<= 8 free keyframes and enough fixed ones for points with 33 and 65 edges: the second and third round of the point loop
+    of ba_linearize_kernel (lane = edge, 32 edges per round) and of the edge strides of ba_update_kernel, lines with 40
+    edges, landmarks with only fixed observers (no pool entry), 2-observation landmarks, plane edges on long tracks."""
+    import ba_data
+    n_kf = n_free + n_fixed
+    prob = ba_data.make_ba_shape_problem(
+        seed, n_free, n_fixed,
+        points=[dict(n=2, k=33), dict(n=2, k=65), dict(n=1, k="all"), dict(n=2, k=64, plane=True), dict(n=2, k=32),
+                dict(n=2, k=4, who="fixed"), dict(n=2, k=2), dict(n=2, k=34, who="one_free"), dict(n=24, k=(3, 9))],
+        lines=[dict(n=2, k=40), dict(n=1, k=3, who="fixed"), dict(n=5, k=(3, 9))] if lines else (), **kw)
+    sh = prob.shape
+    assert list(sh["pt_deg"][:15]) == [33, 33, 65, 65, n_kf - len(kw.get("empty_free", ())), 64, 64, 32, 32, 4, 4, 2, 2, 34, 34]
+    assert list(sh["pt_free_deg"][9:11]) == [0, 0] and list(sh["pt_free_deg"][13:15]) == [1, 1]
+    assert not lines or (list(sh["ln_deg"][:3]) == [40, 40, 3] and sh["ln_free_deg"][2] == 0)
+    return prob
+
+
+_BA_EMU_CASES = {
+    "pt33_pt65_ln40_6free_64fixed": lambda: _ba_long_tracks(5, 6, 64),
+    "pt33_pt65_points_only": lambda: _ba_long_tracks(7, 6, 64, lines=False),
+    "pt33_pt65_stereo_mixed_8free_62fixed_one_empty": lambda: _ba_long_tracks(6, 8, 62, stereo_frac=0.6, empty_free=(7,)),
+}
+
+
+def _emu_solve_equals_oracle(ba_emu, prob, ctas, first=5, second=10):
     import ba_data
     import oracle_api
     orc = oracle_api.Oracle()
-    prob = ba_data.make_ba_problem(3, n_local=4, n_fixed=2, n_points=60, n_lines=12, n_plane_pts=6)
-    o = ba_data.oracle_local_ba(orc, prob)
-    kf, pts, ln, po, lo, it = _emu_ba_solve(ba_emu, prob, ctas=3)
+    o = ba_data.oracle_local_ba(orc, prob, num_first=first, num_second=second)
+    kf, pts, ln, po, lo, it = _emu_ba_solve(ba_emu, prob, first=first, second=second, ctas=ctas)
     assert it == (o.iters_first, o.iters_second, o.lm_tries)                       # same LM path, try for try
     assert np.linalg.norm(kf - o.kf_pose_cw) / np.linalg.norm(o.kf_pose_cw) < 1e-6
     assert np.abs(pts - o.pt_pos_w).max() < 1e-5
     assert np.abs(ln - o.line_plucker[:len(ln)]).max() < 1e-3                      # numeric line Jacobians (delta = 1e-9)
     assert np.array_equal(po, o.pt_edge_outlier[:len(po)]) and np.array_equal(lo, o.line_edge_outlier[:len(lo)])
+
+
+def test_local_ba_kernels_equal_oracle(ba_emu):
+    import ba_data
+    prob = ba_data.make_ba_problem(3, n_local=4, n_fixed=2, n_points=60, n_lines=12, n_plane_pts=6)
+    _emu_solve_equals_oracle(ba_emu, prob, ctas=3)
+
+
+@pytest.mark.parametrize("case,ctas", [("pt33_pt65_ln40_6free_64fixed", 3), ("pt33_pt65_stereo_mixed_8free_62fixed_one_empty", 2)])
+def test_local_ba_kernels_equal_oracle_on_long_tracks(ba_emu, case, ctas):
+    """The same comparison on the shapes make_ba_problem cannot draw (see _ba_long_tracks): every point loop of the
+    linearisation and of the back-substitution takes more than one round of 32 edges.  optimize(3), the outlier round,
+    optimize(5): every kernel and both phases at half the emulation time of the full 5 + 10 iterations."""
+    _emu_solve_equals_oracle(ba_emu, _BA_EMU_CASES[case](), ctas, first=3, second=5)
+
+
+@pytest.mark.parametrize("case,ctas,tol", [("pt33_pt65_ln40_6free_64fixed", 3, 1e-5), ("pt33_pt65_points_only", 1, 1e-13)])
+def test_local_ba_first_try_matches_full_normal_equations(ba_emu, case, ctas, tol):
+    """The reduced camera system S, g, chi2 and lambda of the first real try, as ba_linearize_kernel / ba_reduce_kernel leave
+    them, against the Schur complement of tests/ba_numpy.py's full normal equations in long double (lines: numeric
+    Jacobians with delta = 1e-9 on both sides, hence 1e-5), and the step of ba_solve_kernel by its backward error."""
+    import ba_system_ref as ref
+    prob = _BA_EMU_CASES[case]()
+    n_free = int((prob.kf_fixed == 0).sum())
+    n_pairs = n_free * (n_free + 1) // 2
+    packed, dp, lam = np.zeros(n_pairs * 36 + 12 * n_free + 1), np.zeros(6 * n_free), C.c_double(0.0)
+    ba_emu.emu_ba_capture_try(packed.ctypes.data_as(_P), dp.ctypes.data_as(_P), C.byref(lam))
+    _emu_ba_solve(ba_emu, prob, first=1, second=0, mode=1, ctas=ctas)
+    nS = n_pairs * 36
+    got = dict(S=packed[:nS].reshape(n_pairs, 6, 6), g=packed[nS:nS + 6 * n_free], bp=packed[nS + 6 * n_free:nS + 12 * n_free],
+               chi2=float(packed[-1]), dp=dp, lam=lam.value)
+    ref.check_system(got, prob, n_free, tol)
+    assert np.abs(dp).max() > 1e-4
+    assert ref.backward_error(ref.dense_from_blocks(got["S"], n_free), got["g"], dp, lam.value) < 5e-17
