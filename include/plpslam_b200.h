@@ -851,6 +851,43 @@ PLP_API plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_
 PLP_API plp_status plp_tracker_keyframe_bow(const plp_tracker *t, const int32_t **d_word_id, const int32_t **d_node_id,
                                             const float **d_weight);
 
+/* frame_tracker::robust_match_based_track (module/frame_tracker.cc:192-245) against each frame's reference keyframe, for
+ * the frames whose keyframe track (the preceding plp_tracker_keyframe_track_batch_dev of the same batch) ran and failed:
+ * robust::brute_force_match (Lowe 0.8, no orientation check; frame = side 1) -> the match list in frame keypoint order
+ * -> essential_solver(frm.bearings_, keyfrm->bearings_, matches).find_via_ransac(50, false) -> the inlier matches;
+ * below 20 the frame fails, else pose_optimizer::optimize from last_frm.cam_pose_cw_ -> discard_outliers.  Monocular.
+ * Allocates the scratch for max_batch frames; call it once, outside the hot path (a second call replaces the first).
+ * Refuses a tracker whose kp_capacity exceeds the brute-force matcher's 4096 or the hypothesis kernel's shared memory. */
+PLP_API plp_status plp_tracker_reserve_robust_track(plp_tracker *t);
+/* Follows keyframe_track_batch_dev on the same stream (batch <= that call's batch) and reads the keyframe table it was
+ * given (rows, desc, valid, pos_w, kf_of_frame, local_idx: keep it alive) and the motion and keyframe calls' outputs and
+ * scratch; writes none of them.  d_kf_bearings: keyfrm->bearings_, one row of 3 doubles per keyframe-table row.  The
+ * frame bearings are the undistortion's (distorted tracker) or convert_keypoints_to_bearings of the keypoints.  The
+ * RANSAC sample sets are drawn on the device from `seed` (see plp_tracker_robust_samples).  No host synchronisation.
+ * Outputs (device):
+ *   stage_out[batch]: 1 = the stage ran (keyframe stage 1 and keyframe num_valid < 20; tracking succeeded iff
+ *     num_valid >= 20), else 0;
+ *   kf_matched_out[batch x kp_capacity]: the keyframe row each keypoint keeps after discard_outliers, or -1;
+ *   num_bf_matches_out[batch]: the brute-force match count, num_robust_matches_out[batch]: the RANSAC inliers among
+ *     them (0 if the solution is not valid) (both 0 where the stage did not run);
+ *   pose_out[batch x 16]: the optimiser result, or pose_last where it did not run or found fewer than 20 robust matches;
+ *   num_valid_out, n_inliers_out, lm_iters_out [batch] (0 where the optimiser did not run);
+ *   status_out[batch]: the keyframe call's status; a frame with status != 0 fails like a track with no match.
+ * Without a reservation, with no preceding keyframe track since the last motion track, or with batch above its batch:
+ * PLP_ERR_INVALID and nothing is launched.  A following local_map_track_batch_dev of the same batch starts each frame
+ * that ran this stage from its result (see INTEGRATION.md). */
+PLP_API plp_status plp_tracker_robust_track_batch_dev(plp_tracker *t, int batch, const double *d_kf_bearings,
+                                                      uint64_t seed, int32_t *d_stage_out, int32_t *d_kf_matched_out,
+                                                      int32_t *d_num_bf_matches_out, int32_t *d_num_robust_matches_out,
+                                                      double *d_pose_out, int32_t *d_num_valid_out,
+                                                      int32_t *d_n_inliers_out, int32_t *d_lm_iters_out,
+                                                      int32_t *d_status_out);
+/* The RANSAC sample sets of the most recent robust_track_batch_dev (max_batch x 50 x 8 indices into the frame's
+ * brute-force match list, -1 where none were drawn): a device pointer owned by the tracker, valid once its stream has
+ * reached that call.  They are util::create_random_array(8, 0, n - 1) over a counter-based generator keyed by
+ * (seed, frame, hypothesis); see csrc/ransac_sample.h. */
+PLP_API plp_status plp_tracker_robust_samples(const plp_tracker *t, const int32_t **d_samples);
+
 /* ------------------------------------------------------------------------ */
 /* local bundle adjustment (optimize/local_bundle_adjuster*.cc)               */
 /* ------------------------------------------------------------------------ */

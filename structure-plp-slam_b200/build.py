@@ -38,6 +38,7 @@ FILE_FLAGS = {
     "camera.cu": NO_FMA,
     "local_map.cu": NO_FMA,
     "keyframe_track.cu": NO_FMA,
+    "robust_track.cu": NO_FMA,
 }
 
 

@@ -4,7 +4,7 @@
 #include <stddef.h>
 #include <stdint.h>
 
-#include "essmath.h"
+#include "essential_common.cuh"
 
 namespace plp {
 
@@ -31,39 +31,15 @@ struct EssJob {
 
 // inlier test of every match against E (all threads), then the ordered float sum (thread 0); returns the score to thread 0
 __device__ float check_inliers_cta(const EssJob &J, const double *E, uint8_t *inlier, float *res) {
-    const int tid = threadIdx.x;
-    for (int i = tid; i < J.num_matches; i += kEssThreads) {
-        float s2, s1;
-        int add1;
-        inlier[i] = (uint8_t)ess_check_match(E, J.b1 + 3 * (size_t)J.matches[2 * i], J.b2 + 3 * (size_t)J.matches[2 * i + 1],
-                                             &s2, &add1, &s1);
-        res[2 * i] = s2;
-        res[2 * i + 1] = add1 ? s1 : -1.0f;  // -1 marks "not added" (residuals are absolute values, never negative)
-    }
-    __syncthreads();
-    float score = 0;
-    if (tid == 0) {
-        for (int i = 0; i < J.num_matches; ++i) {
-            score += res[2 * i];
-            const float s1 = res[2 * i + 1];
-            if (!(s1 == -1.0f)) score += s1;
-        }
-    }
-    return score;
+    return ess_score_cta<kEssThreads>(J.b1, J.b2, J.matches, J.num_matches, E, inlier, res);
 }
 
 __global__ void __launch_bounds__(kEssThreads) essential_hypothesis_kernel(EssJob J) {
     __shared__ double sE[9];
     const int iter = blockIdx.x, tid = threadIdx.x;
     if (tid == 0) {
-        double ata[81];
-        for (int k = 0; k < 81; ++k) ata[k] = 0.0;
-        for (int i = 0; i < 8; ++i) {  // :72-78
-            const int idx = J.samples[iter * 8 + i];
-            ess_accumulate(ata, J.b1 + 3 * (size_t)J.matches[2 * idx], J.b2 + 3 * (size_t)J.matches[2 * idx + 1]);
-        }
         double E[9];
-        ess_solve(ata, E);  // :81
+        ess_hypothesis(J.b1, J.b2, J.matches, J.samples + iter * 8, E);  // :72-81
         for (int k = 0; k < 9; ++k) {
             sE[k] = E[k];
             J.E[iter * 9 + k] = E[k];
@@ -81,15 +57,8 @@ __global__ void __launch_bounds__(kEssThreads) essential_select_kernel(EssJob J)
     const int tid = threadIdx.x;
     if (tid == 0) {
         s_cnt = 0;
-        double best_score = 0.0;
-        int best = -1;
-        for (int it = 0; it < J.num_iter; ++it) {  // :87-92, in iteration order
-            const float sc = J.score[it];
-            if (best_score < (double)sc) {
-                best_score = (double)sc;
-                best = it;
-            }
-        }
+        double best_score;
+        const int best = ess_first_best(J.score, J.num_iter, &best_score);  // :87-92
         s_best = best;
         *J.best_score = best_score;
         for (int k = 0; k < 9; ++k) J.best_E[k] = best >= 0 ? J.E[best * 9 + k] : 0.0;

@@ -130,6 +130,7 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     t->has_kf = false;
+    t->has_rb = false;
     const TrackDev &M = t->motion;
     KfDev D = *t->kf;
     D.batch = batch;
@@ -190,6 +191,7 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
     K.kf_of_frame = kf->kf_of_frame;
     K.local_idx = kf->local_idx;
     K.local_idx_offsets = kf->local_idx_offsets;
+    t->kf_table = *kf;
     t->kf_batch = batch;
     t->has_kf = true;
     return PLP_OK;

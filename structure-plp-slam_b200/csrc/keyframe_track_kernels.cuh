@@ -81,6 +81,10 @@ __device__ __forceinline__ bool frame_active(const KfDev &D, int b) {
     return D.stage[b] != 0 && D.status[b] == kStatusOk;
 }
 
+// The kernels have internal linkage, as essential_kernels.cuh's do: robust_track.cu launches the gather and finish
+// kernels as well, over its own matches.
+namespace {
+
 // tracking_module.cc:608-637: the frames the reference hands to bow_match_based_track
 __global__ void __launch_bounds__(kPrepThreads) kf_prep_kernel(KfDev D) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
@@ -250,6 +254,8 @@ __global__ void __launch_bounds__(kThreads) kf_finish_kernel(KfDev D) {
                                                  D.obs_outlier + base, D.obs_kp + base, D.matched + base);
     if (threadIdx.x == 0) D.num_valid[b] = valid;
 }
+
+}  // namespace
 
 }  // namespace kt
 

@@ -99,6 +99,8 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
                 "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
     PLP_REQUIRE(!t->has_kf || batch <= t->kf_batch,
                 "the batch must not exceed that of the plp_tracker_keyframe_track_batch_dev that followed the motion track");
+    PLP_REQUIRE(!t->has_rb || batch <= t->rb_batch,
+                "the batch must not exceed that of the plp_tracker_robust_track_batch_dev that followed the keyframe track");
     PLP_REQUIRE(margin > 0.0f, "margin");
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
@@ -119,6 +121,7 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.obs_last = M.obs_last;
     for (int l = 0; l < 16; ++l) D.inv_level_sigma_sq[l] = M.inv_level_sigma_sq[l];
     if (t->has_kf) D.kf = t->kf_track;  // else D.kf.stage stays null: every frame starts from its motion track
+    if (t->has_rb) D.rb = t->rb_track;  // else D.rb.stage stays null: no frame starts from a robust track
     D.pos_w = local->pos_w;
     D.normal = local->obs_mean_normal;
     D.min_d = local->min_valid_dist;

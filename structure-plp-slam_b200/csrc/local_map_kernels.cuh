@@ -1,7 +1,8 @@
 // local_map_kernels.cuh -- device code of the batched local-map stage of tracking (local_map.cu launches it):
 // tracking_module::optimize_current_frame_with_local_map (tracking_module.cc:732-835) for the frames whose
 // motion_based_track succeeded, or, after a keyframe-track call of the same batch (keyframe_track.cu), whose
-// bow_match_based_track did; monocular points:
+// bow_match_based_track did, or, after a robust-track call of the same batch (robust_track.cu), whose
+// robust_match_based_track did; monocular points:
 //   search_local_landmarks (:908-984) = exclusion of the landmarks the motion track matched, frame::can_observe
 //   (data/frame.cc:797-824) and projection::match_frame_and_landmarks (margin, Lowe ratio 0.8)
 //   -> pose_optimizer::optimize -> drop the outliers and count the tracked landmarks (:762-784).
@@ -59,8 +60,8 @@ struct LocalDev {
     const PoseJob *motion_jobs;        // batch: n_pts = observations of pose-opt #1
     const int32_t *obs_last;           // batch x cap: last-frame row of each observation of pose-opt #1
     float inv_level_sigma_sq[kMaxLevels];
-    // the keyframe track of the same batch; kf.stage == nullptr without one
-    KeyframeTrack kf;
+    // the keyframe and robust tracks of the same batch; kf.stage / rb.stage == nullptr without one
+    KeyframeTrack kf, rb;
     // the local maps (rows of frame b: [offsets[b], offsets[b + 1]))
     const double *pos_w, *normal;
     const float *min_d, *max_d, *max_raw;
@@ -95,14 +96,18 @@ struct LocalDev {
     int32_t *num_tracked, *n_inliers, *lm_iters, *status;  // batch
 };
 
-// The tracker whose result the frame starts from: the keyframe track where it ran (stage 1), else the motion track.
-// Its matches are rows of the keyframe or of the last frame.
+// The tracker whose result the frame starts from: the robust track where it ran, else the keyframe track where it ran
+// (stage 1), else the motion track.  The robust track runs only where the keyframe track ran, and both match against
+// rows of the same keyframe; the motion track's matches are rows of the last frame.
 __device__ __forceinline__ bool kf_tracked(const LocalDev &D, int b) { return D.kf.stage && D.kf.stage[b]; }
+__device__ __forceinline__ const KeyframeTrack &kf_record(const LocalDev &D, int b) {
+    return D.rb.stage && D.rb.stage[b] ? D.rb : D.kf;
+}
 __device__ __forceinline__ int tracked_num_valid(const LocalDev &D, int b) {
-    return kf_tracked(D, b) ? D.kf.num_valid[b] : D.motion_num_valid[b];
+    return kf_tracked(D, b) ? kf_record(D, b).num_valid[b] : D.motion_num_valid[b];
 }
 __device__ __forceinline__ const double *tracked_pose(const LocalDev &D, int b) {
-    return (kf_tracked(D, b) ? D.kf.pose : D.motion_pose) + 16 * (size_t)b;
+    return (kf_tracked(D, b) ? kf_record(D, b).pose : D.motion_pose) + 16 * (size_t)b;
 }
 
 // the frame runs the stage: its tracker succeeded and its inputs are in range
@@ -121,21 +126,23 @@ __global__ void __launch_bounds__(kThreads) local_prep_kernel(LocalDev D) {
     __shared__ int s_bad;
     const int b = blockIdx.x, tid = threadIdx.x;
     const int l0 = D.offsets[b], m = D.offsets[b + 1] - l0;
-    const bool kf = kf_tracked(D, b), kf_ok = kf && D.kf.status[b] == 0;
+    const bool kf = kf_tracked(D, b);
+    const KeyframeTrack &K = kf_record(D, b);
+    const bool kf_ok = kf && K.status[b] == 0;
     // the rows the tracker matched against, and their local-list indices: the keyframe's or the last frame's
     const int32_t *row_local = D.last_local_idx;
     int r0 = D.last_offsets[b], r1 = D.last_offsets[b + 1];
     bool rows_ok = true;
     if (kf) {
         r0 = r1 = 0;
-        row_local = D.kf.local_idx;
+        row_local = K.local_idx;
         if (kf_ok) {  // frame b's local_idx block has one entry per row of its keyframe
-            const int k = D.kf.kf_of_frame[b];
-            rows_ok = D.kf.local_idx && D.kf.local_idx_offsets[b + 1] - D.kf.local_idx_offsets[b] ==
-                                            D.kf.kf_row_offsets[k + 1] - D.kf.kf_row_offsets[k];
+            const int k = K.kf_of_frame[b];
+            rows_ok = K.local_idx && K.local_idx_offsets[b + 1] - K.local_idx_offsets[b] ==
+                                         K.kf_row_offsets[k + 1] - K.kf_row_offsets[k];
             if (rows_ok) {
-                r0 = D.kf.local_idx_offsets[b];
-                r1 = D.kf.local_idx_offsets[b + 1];
+                r0 = K.local_idx_offsets[b];
+                r1 = K.local_idx_offsets[b + 1];
             }
         }
     }
@@ -157,7 +164,7 @@ __global__ void __launch_bounds__(kThreads) local_prep_kernel(LocalDev D) {
     const int status = !fits ? kStatusCapacity : (s_bad ? kStatusLastLocalIdx : kStatusOk);
     const bool active = tracked_num_valid(D, b) >= kNumMatchesThr && status == kStatusOk;
     // the landmarks the frame keeps from its tracker; they are the matcher's claimed keypoints
-    const int32_t *tracked_matched = kf ? D.kf.matched : D.motion_matched;
+    const int32_t *tracked_matched = kf ? K.matched : D.motion_matched;
     for (int i = tid; i < n; i += kThreads) {
         const int q = active ? tracked_matched[base + i] : -1;
         D.matched[base + i] = q;
@@ -167,8 +174,8 @@ __global__ void __launch_bounds__(kThreads) local_prep_kernel(LocalDev D) {
     // Every landmark the tracker matched is excluded, the outliers of pose-opt #1 included: discard_outliers stamps
     // identifier_in_local_lm_search_ on those (frame_tracker.cc:273-278), search_local_landmarks on the rest (:910-926).
     if (active) {
-        const int n1 = (kf ? D.kf.posejobs : D.motion_jobs)[b].n_pts;
-        const int32_t *obs_row = (kf ? D.kf.obs_row : D.obs_last) + base;
+        const int n1 = (kf ? K.posejobs : D.motion_jobs)[b].n_pts;
+        const int32_t *obs_row = (kf ? K.obs_row : D.obs_last) + base;
         for (int k = tid; k < n1; k += kThreads) {
             const int li = row_local[r0 + obs_row[k]];
             if (li >= 0) D.excl[lbase + li] = 1;
@@ -260,8 +267,9 @@ __global__ void __launch_bounds__(kThreads) local_gather_kernel(LocalDev D) {
     const int l0 = D.offsets[b];
     // the positions of the tracker's matches: keyframe rows or last-frame rows
     const bool kf = kf_tracked(D, b);
+    const KeyframeTrack &K = kf_record(D, b);
     const double *row_pos_w =
-        kf ? D.kf.kf_pos_w + 3 * (size_t)(active ? D.kf.kf_row_offsets[D.kf.kf_of_frame[b]] : 0)
+        kf ? K.kf_pos_w + 3 * (size_t)(active ? K.kf_row_offsets[K.kf_of_frame[b]] : 0)
            : D.last_pos_w + 3 * (size_t)D.last_offsets[b];
     if (active) {  // the local row each keypoint matched (projection.cc:115: frm.landmarks_.at(best_idx) = local_lm)
         const int m = D.offsets[b + 1] - l0;

@@ -248,6 +248,7 @@ void plp_tracker_destroy(plp_tracker *t) {
     if (t->d_block) cudaFree(t->d_block);
     if (t->d_local) cudaFree(t->d_local);
     if (t->d_kf) cudaFree(t->d_kf);
+    if (t->d_rb) cudaFree(t->d_rb);
     delete t;
 }
 
@@ -265,6 +266,7 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
     plp_ctx *ctx = t->ctx;
     t->has_motion = false;
     t->has_kf = false;
+    t->has_rb = false;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     TrackDev T = t->dev;
     T.batch = batch;

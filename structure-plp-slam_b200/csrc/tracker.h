@@ -1,6 +1,6 @@
 // tracker.h -- internal: the state of a plp_tracker, shared by pipeline.cu (motion_based_track), keyframe_track.cu
-// (bow_match_based_track) and local_map.cu (optimize_current_frame_with_local_map), which read what the motion call
-// left on the device.
+// (bow_match_based_track), robust_track.cu (robust_match_based_track) and local_map.cu
+// (optimize_current_frame_with_local_map), which read what the earlier calls of the batch left on the device.
 #pragma once
 #include <memory>
 
@@ -17,6 +17,9 @@ struct LocalDev;  // local_map_kernels.cuh
 }
 namespace kt {
 struct KfDev;  // keyframe_track_kernels.cuh
+}
+namespace rt {
+struct RtDev;  // robust_track_kernels.cuh
 }
 
 struct TrackDev {
@@ -86,8 +89,16 @@ struct plp_tracker {
     int max_keyframes = 0, max_kf_points = 0;
     uint8_t *d_kf = nullptr;         // one allocation, carved by keyframe_track.cu
     std::shared_ptr<plp::kt::KfDev> kf;
-    // the keyframe_track_batch_dev that followed the most recent motion track, for the local-map stage
+    // the keyframe_track_batch_dev that followed the most recent motion track, for the robust and local-map stages
     plp::KeyframeTrack kf_track;
+    plp_track_keyframe kf_table;     // the keyframe table that call was given
     int kf_batch = 0;
     bool has_kf = false;
+    // robust tracking (plp_tracker_reserve_robust_track); d_rb == nullptr until reserved
+    uint8_t *d_rb = nullptr;         // one allocation, carved by robust_track.cu
+    std::shared_ptr<plp::rt::RtDev> rb;
+    // the robust_track_batch_dev that followed the most recent keyframe track, for the local-map stage
+    plp::KeyframeTrack rb_track;
+    int rb_batch = 0;
+    bool has_rb = false;
 };

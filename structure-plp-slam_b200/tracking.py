@@ -1,8 +1,9 @@
-"""Device-resident batched front-end: ORB extraction + motion-based tracking (+ optionally the keyframe tracker and the
-local-map stage) without leaving HBM.
+"""Device-resident batched front-end: ORB extraction + motion-based tracking (+ optionally the keyframe and robust
+trackers and the local-map stage) without leaving HBM.
 
 Thin ctypes layer over plp_orb_extract_batch_dev + plp_tracker_motion_track_batch_dev (+
-plp_tracker_keyframe_track_batch_dev, plp_tracker_local_map_track_batch_dev); used by bench.py and the pipeline parity
+plp_tracker_keyframe_track_batch_dev, plp_tracker_robust_track_batch_dev, plp_tracker_local_map_track_batch_dev); used
+by bench.py and the pipeline parity
 tests.  No compute here.
 """
 from __future__ import annotations
@@ -162,6 +163,8 @@ class FrontEnd:
         self._kf_bufs = []
         self._kf = None
         self._kf_out = None
+        self._kf_bearings = None
+        self._rb_out = None
         self._last_bufs = []
         self._last = None
         self._last_pinned = []   # host copies of the last-frame arrays (end-to-end path: uploaded every step)
@@ -174,6 +177,7 @@ class FrontEnd:
             b.free()
         self._local_bufs = []
         self._kf_bufs = []
+        self._kf_bearings = None
         if self._trk is not None:
             self.lib.plp_tracker_destroy(self._trk)
             self._trk = None
@@ -255,7 +259,8 @@ class FrontEnd:
 
     def set_keyframes(self, keyframes, kf_of_frame, local_idx=None):
         """keyframes[k]: dict(desc[n,32], angle[n] (keypts_[i].angle), valid[n]|None (lm && !will_be_erased()),
-        pos_w[n,3], fv=(node_ids, offsets, indices) (bow_feat_vec_ flattened, as capi.fold_bow returns it));
+        pos_w[n,3], fv=(node_ids, offsets, indices) (bow_feat_vec_ flattened, as capi.fold_bow returns it),
+        bearings[n,3] (keyfrm->bearings_; optional, read by track_robust only));
         kf_of_frame[b]: frame b's reference keyframe.  local_idx (optional, for track_local_map after track_keyframe):
         per frame, one entry per row of its keyframe -- that landmark's index in the frame's local list, or -1."""
         for b in self._kf_bufs:
@@ -287,6 +292,21 @@ class FrontEnd:
         self._kf_bufs = [DeviceBuffer.from_array(self.ctx, a) for a in arrays]
         ptrs = [b.ptr for b in self._kf_bufs] + [None] * (12 - len(self._kf_bufs))
         self._kf = TrackKeyframe(len(keyframes), *ptrs)
+        self._kf_bearings = None
+        if keyframes and all(k.get("bearings") is not None for k in keyframes):
+            self._kf_bearings = DeviceBuffer.from_array(self.ctx, cat("bearings", np.float64, (3,)))
+            self._kf_bufs.append(self._kf_bearings)
+
+    def reserve_robust_track(self):
+        """Scratch of track_robust (outside the hot path), and its outputs."""
+        self.ctx._check(self.lib.plp_tracker_reserve_robust_track(self._trk))
+        B = self.max_batch
+        if self._rb_out is None:
+            self._rb_out = dict(stage=DeviceBuffer(self.ctx, B * 4), matched=DeviceBuffer(self.ctx, B * self.cap * 4),
+                                num_bf=DeviceBuffer(self.ctx, B * 4), num_robust=DeviceBuffer(self.ctx, B * 4),
+                                pose=DeviceBuffer(self.ctx, B * 128), num_valid=DeviceBuffer(self.ctx, B * 4),
+                                n_inliers=DeviceBuffer(self.ctx, B * 4), lm_iters=DeviceBuffer(self.ctx, B * 4),
+                                status=DeviceBuffer(self.ctx, B * 4))
 
     # -- end-to-end path: every input of a step comes from pinned host memory, every result goes back ----
     def stage_host_io(self, imgs: np.ndarray):
@@ -397,6 +417,18 @@ class FrontEnd:
             o["num_bow"].ptr, o["pose"].ptr, o["num_valid"].ptr, o["n_inliers"].ptr, o["lm_iters"].ptr,
             o["status"].ptr))
 
+    def track_robust(self, batch: int, seed: int = 0):
+        """robust_match_based_track for the frames of the preceding track_keyframe() that ran that stage and failed,
+        against the same keyframe table (whose keyframes need "bearings"); RANSAC samples drawn on the device from
+        `seed` (tracking stream)."""
+        o = self._rb_out
+        if o is None or self._kf_bearings is None:
+            raise PlpError("track_robust needs reserve_robust_track() and set_keyframes() with keyframe bearings first")
+        self.ctx._check(self.lib.plp_tracker_robust_track_batch_dev(
+            self._trk, C.c_int(batch), self._kf_bearings.ptr, C.c_uint64(seed), o["stage"].ptr, o["matched"].ptr,
+            o["num_bf"].ptr, o["num_robust"].ptr, o["pose"].ptr, o["num_valid"].ptr, o["n_inliers"].ptr,
+            o["lm_iters"].ptr, o["status"].ptr))
+
     # -- results --------------------------------------------------------------------------------------
     def _after_tracking(self):
         """The downloads below run on the extraction stream; the tracking outputs are written on the tracking stream."""
@@ -469,6 +501,30 @@ class FrontEnd:
                     lm_iters=o["lm_iters"].download(np.int32, (batch,)),
                     status=o["status"].download(np.int32, (batch,)),
                     bow=[tuple(a[b, :n[b]].copy() for a in bow) for b in range(batch)])
+
+    def download_robust_tracking(self, batch: int):
+        """Results of track_robust: per frame the stage flag, the keyframe row kept on each keypoint, the brute-force
+        and robust (RANSAC inlier) match counts, pose, num_valid, n_inliers, LM iterations, status, and the 50 x 8
+        RANSAC sample sets (indices into the frame's brute-force match list, -1 where none were drawn)."""
+        self._after_tracking()
+        n = self.d_n.download(np.int32, (batch,))
+        o = self._rb_out
+        matched = o["matched"].download(np.int32, (self.max_batch, self.cap))[:batch]
+        p = C.c_void_p()
+        self.ctx._check(self.lib.plp_tracker_robust_samples(self._trk, C.byref(p)))
+        samples = np.zeros((self.max_batch, 50, 8), np.int32)
+        self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, samples.ctypes.data_as(_P), p,
+                                                  C.c_size_t(samples.nbytes)))
+        return dict(stage=o["stage"].download(np.int32, (batch,)),
+                    matched=[matched[b, :n[b]].copy() for b in range(batch)],
+                    num_bf_matches=o["num_bf"].download(np.int32, (batch,)),
+                    num_robust_matches=o["num_robust"].download(np.int32, (batch,)),
+                    pose=o["pose"].download(np.float64, (batch, 4, 4)),
+                    num_valid=o["num_valid"].download(np.int32, (batch,)),
+                    n_inliers=o["n_inliers"].download(np.int32, (batch,)),
+                    lm_iters=o["lm_iters"].download(np.int32, (batch,)),
+                    status=o["status"].download(np.int32, (batch,)),
+                    samples=samples[:batch].copy())
 
     def download_tracking(self, batch: int):
         self._after_tracking()
