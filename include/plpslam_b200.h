@@ -822,7 +822,8 @@ typedef struct plp_track_keyframe { /* device pointers except num_keyframes; key
 } plp_track_keyframe;
 
 /* Allocates the keyframe-track scratch for max_batch frames whose keyframes hold up to max_keyframe_points rows each, in
- * tables of up to max_keyframes keyframes; call it once, outside the hot path. */
+ * tables of up to max_keyframes keyframes; call it once, outside the hot path.  A kp_capacity whose feature-vector kernel
+ * needs more shared memory (12 bytes per keypoint) than the device offers: PLP_ERR_CAPACITY, nothing allocated. */
 PLP_API plp_status plp_tracker_reserve_keyframe_track(plp_tracker *t, int max_keyframes, int max_keyframe_points);
 /* Follows motion_track_batch_dev on the same stream (batch <= that call's batch) and reads its inputs, outputs and
  * scratch; writes none of them.  Frame b runs the stage iff d_motion_valid[b] == 0 (NULL: all 1; the reference's
@@ -857,7 +858,8 @@ PLP_API plp_status plp_tracker_keyframe_bow(const plp_tracker *t, const int32_t 
  * -> essential_solver(frm.bearings_, keyfrm->bearings_, matches).find_via_ransac(50, false) -> the inlier matches;
  * below 20 the frame fails, else pose_optimizer::optimize from last_frm.cam_pose_cw_ -> discard_outliers.  Monocular.
  * Allocates the scratch for max_batch frames; call it once, outside the hot path (a second call replaces the first).
- * Refuses a tracker whose kp_capacity exceeds the brute-force matcher's 4096 or the hypothesis kernel's shared memory. */
+ * Refuses a tracker whose kp_capacity exceeds the brute-force matcher's 4096 (PLP_ERR_INVALID) or the hypothesis
+ * kernel's shared memory (PLP_ERR_CAPACITY), before allocating anything. */
 PLP_API plp_status plp_tracker_reserve_robust_track(plp_tracker *t);
 /* Follows keyframe_track_batch_dev on the same stream (batch <= that call's batch) and reads the keyframe table it was
  * given (rows, desc, valid, pos_w, kf_of_frame, local_idx: keep it alive) and the motion and keyframe calls' outputs and

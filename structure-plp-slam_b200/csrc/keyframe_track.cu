@@ -5,11 +5,11 @@
 // for the frames of the tracker's most recent plp_tracker_motion_track_batch_dev that the reference hands to it (motion
 // model unusable, or motion track failed), on the same stream and without leaving HBM.  It reads that call's inputs and
 // scratch (tracker.h) and writes separate outputs.  Device code: keyframe_track_kernels.cuh; the BoW matcher
-// (bow_match_kernel) and the pose optimiser are the existing ones, the vocabulary descent is bow_transform_kernel's.
+// (bow_match_kernel) and the tail (track_common.cuh) are the existing ones, the vocabulary descent is
+// bow_transform_kernel's.
 #include "common.cuh"
 #include "bow_vocab.h"
 #include "keyframe_track_kernels.cuh"
-#include "pose_kernels.cuh"
 #include "tracker.h"
 
 namespace plp {
@@ -55,23 +55,13 @@ plp_status plp_tracker_reserve_keyframe_track(plp_tracker *t, int max_keyframes,
     PLP_REQUIRE(t, "null pointer");
     PLP_REQUIRE(max_keyframes >= 1 && max_keyframe_points >= 1, "max_keyframes / max_keyframe_points");
     PLP_CUDA_TRY(cudaSetDevice(t->ctx->device));
-    // The feature-vector kernel's dynamic shared memory, next to its static shared memory, within the opt-in limit.  The
-    // attribute is per kernel, not per tracker: it allows the most any tracker can ask for.
-    const size_t smem = job_smem(t->cap);
-    int optin = 0;
-    cudaFuncAttributes fa;
-    PLP_CUDA_TRY(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, t->ctx->device));
-    PLP_CUDA_TRY(cudaFuncGetAttributes(&fa, kt::kf_job_kernel));
-    PLP_REQUIRE(smem + fa.sharedSizeBytes <= (size_t)optin,
-                "kp_capacity too large for the feature-vector kernel's shared memory");
-    PLP_CUDA_TRY(cudaFuncSetAttribute(kt::kf_job_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                      optin - (int)fa.sharedSizeBytes));
+    PLP_SMEM_OPTIN(kt::kf_job_kernel, job_smem(t->cap));  // the feature-vector kernel's cap x 12 bytes
     if (t->d_kf) {  // a second reservation replaces the first once the stream has stopped using it
         PLP_CUDA_TRY(cudaStreamSynchronize(t->ctx->stream));
         cudaFree(t->d_kf);
         t->d_kf = nullptr;
         t->max_keyframes = t->max_kf_points = 0;
-        t->has_kf = false;
+        t->invalidate_from(kStageKeyframe);
     }
     // the scratch of every later call, bound once (B frames, C keypoints, R keyframe rows)
     const size_t B = t->max_batch, C = t->cap, R = max_keyframe_points;
@@ -90,11 +80,12 @@ plp_status plp_tracker_reserve_keyframe_track(plp_tracker *t, int max_keyframes,
     L.out(D->choice, B * R);
     L.out(D->m21, B * R);
     L.out(D->bjobs, B);
-    L.out(D->posejobs, B);
-    L.out(D->obs, B * C);
-    L.out(D->obs_kp, B * C);
-    L.out(D->obs_row, B * C);
-    L.out(D->obs_outlier, B * C);
+    TrackTail J = t->tail[kStageMotion];  // the tracker's cap and inv_level_sigma_sq; this stage's scratch
+    L.out(J.posejobs, B);
+    L.out(J.obs, B * C);
+    L.out(J.obs_kp, B * C);
+    L.out(J.obs_row, B * C);
+    L.out(J.obs_outlier, B * C);
     if (alloc(t->ctx, L, &t->d_kf, false) != cudaSuccess) {
         set_error("tracker: cudaMalloc(%zu) for keyframe tracking failed", L.bytes());
         return PLP_ERR_CUDA;
@@ -104,6 +95,8 @@ plp_status plp_tracker_reserve_keyframe_track(plp_tracker *t, int max_keyframes,
     D->cap = t->cap;
     D->max_kf_points = max_keyframe_points;
     t->kf = D;
+    t->kf_choice = D->choice;
+    t->tail[kStageKeyframe] = J;
     return PLP_OK;
 }
 
@@ -124,33 +117,26 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
     PLP_REQUIRE(kf->num_keyframes >= 0 && kf->num_keyframes <= t->max_keyframes,
                 "num_keyframes exceeds the reserved max_keyframes");
     PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
-    PLP_REQUIRE(t->has_motion && batch <= t->motion.batch,
+    PLP_REQUIRE(t->covers(kStageMotion, batch),
                 "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
     PLP_REQUIRE(vocab->ctx->device == t->ctx->device, "the vocabulary lives on another device");
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    t->has_kf = false;
-    t->has_rb = false;
+    t->invalidate_from(kStageKeyframe);
     const TrackDev &M = t->motion;
     KfDev D = *t->kf;
     D.batch = batch;
     D.num_keyframes = kf->num_keyframes;
     D.n_kp = M.n_kp;
-    D.x = M.x;
-    D.y = M.y;
     D.angle = M.angle;
-    D.octave = M.octave;
     D.desc = M.desc;
-    D.motion_num_valid = M.num_valid;
-    D.pose_last = M.pose_last;
-    for (int l = 0; l < kt::kMaxLevels; ++l) D.inv_level_sigma_sq[l] = M.inv_level_sigma_sq[l];
+    D.motion_num_valid = t->record[kStageMotion].num_valid;
     D.motion_valid = d_motion_valid;
     D.kf_of_frame = kf->kf_of_frame;
     D.row_offsets = kf->row_offsets;
     D.kf_desc = kf->desc;
     D.kf_angle = kf->angle;
     D.kf_valid = kf->valid;
-    D.kf_pos_w = kf->pos_w;
     D.fv_offsets = kf->fv_offsets;
     D.node_ids = kf->node_ids;
     D.node_begin = kf->node_begin;
@@ -159,10 +145,22 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
     D.status = d_status_out;
     D.matched = d_kf_matched_out;
     D.num_bow = (uint32_t *)d_num_bow_matches_out;
-    D.pose = d_pose_out;
-    D.num_valid = d_num_valid_out;
-    D.n_inliers = d_n_inliers_out;
-    D.lm_iters = d_lm_iters_out;
+    // pose-opt from last_frm.cam_pose_cw_ over the frames with 20 BoW matches (frame_tracker.cc:138-169)
+    TrackTail J = t->tail[kStageKeyframe];
+    J.n_kp = M.n_kp;
+    J.x = M.x;
+    J.y = M.y;
+    J.octave = M.octave;
+    J.count = d_num_bow_matches_out;
+    J.stage = d_stage_out;
+    J.status = d_status_out;
+    J.rows = TrackRows{kf->pos_w, kf->row_offsets, kf->kf_of_frame};
+    J.pose_in = M.pose_last;
+    J.matched = d_kf_matched_out;
+    J.pose = d_pose_out;
+    J.num_valid = d_num_valid_out;
+    J.n_inliers = d_n_inliers_out;
+    J.lm_iters = d_lm_iters_out;
 
     PLP_LAUNCH(ctx, kt::kf_prep_kernel, div_up(batch, kt::kPrepThreads), kt::kPrepThreads, 0, D);
     PLP_CHECK_LAUNCH();
@@ -171,29 +169,9 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
     PLP_CHECK_LAUNCH();
     PLP_LAUNCH(ctx, bow_match_kernel, batch, kMatchThreads, 0, D.bjobs, kt::kLoweRatio, 1);
     PLP_CHECK_LAUNCH();
-    PLP_LAUNCH(ctx, kt::kf_gather_kernel, batch, kt::kThreads, 0, D);
-    PLP_CHECK_LAUNCH();
-    plp_pose_opt_cfg cfg{4, 10};
-    PLP_TRY(launch_pose_opt(ctx, D.posejobs, batch, t->cap, t->cam, cfg));
-    PLP_LAUNCH(ctx, kt::kf_finish_kernel, batch, kt::kThreads, 0, D);
-    PLP_CHECK_LAUNCH();
-
-    KeyframeTrack &K = t->kf_track;
-    K.stage = d_stage_out;
-    K.status = d_status_out;
-    K.matched = d_kf_matched_out;
-    K.pose = d_pose_out;
-    K.num_valid = d_num_valid_out;
-    K.posejobs = D.posejobs;
-    K.obs_row = D.obs_row;
-    K.kf_pos_w = kf->pos_w;
-    K.kf_row_offsets = kf->row_offsets;
-    K.kf_of_frame = kf->kf_of_frame;
-    K.local_idx = kf->local_idx;
-    K.local_idx_offsets = kf->local_idx_offsets;
+    PLP_TRY(launch_track_tail(ctx, J, batch, t->cam));
     t->kf_table = *kf;
-    t->kf_batch = batch;
-    t->has_kf = true;
+    t->set_record(kStageKeyframe, batch, J, kf->local_idx, kf->local_idx_offsets);
     return PLP_OK;
 }
 

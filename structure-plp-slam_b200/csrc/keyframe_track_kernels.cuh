@@ -11,27 +11,23 @@
 //                        blocks of the other frames return at once
 //   kf_job_kernel        one CTA per frame: the frame's bow_feat_vec_, the merge-join with the keyframe's node list,
 //                        the BowJob (side 1 = keyframe, side 2 = frame)
-//   kf_gather_kernel     one CTA per frame: the observations of the pose optimisation in keypoint order
-//   kf_finish_kernel     one CTA per frame: discard_outliers
+// then the tail of track_common.cuh: count = the BoW matches, rows = the keyframes', from last_frm.cam_pose_cw_.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
 
 #include "../../include/plpslam_b200.h"
 #include "bow_kernels.cuh"
-#include "pose_jobs.h"
 #include "track_common.cuh"
 
 namespace plp {
 
 namespace kt {
 
-constexpr int kThreads = 256;         // job / gather / finish: one CTA per frame
+constexpr int kThreads = 256;         // job: one CTA per frame
 constexpr int kPrepThreads = 128;
-constexpr int kNumMatchesThr = 20;    // frame_tracker::num_matches_thr_
 constexpr float kLoweRatio = 0.7f;    // frame_tracker.cc:130: bow_tree bow_matcher(0.7, true)
 constexpr int kLevelsUp = 4;          // frame::compute_bow: transform(..., 4)
-constexpr int kMaxLevels = 16;
 
 enum : int32_t { kStatusOk = 0, kStatusCapacity = 1, kStatusKeyframe = 2 };
 
@@ -39,19 +35,15 @@ struct KfDev {
     int batch, cap, num_keyframes, max_kf_points;
     // the motion track of the same batch (tracker state)
     const int32_t *n_kp;
-    const float *x, *y, *angle;        // undistorted keypoints, SoA (batch x cap)
-    const int32_t *octave;
+    const float *angle;                // batch x cap
     const uint8_t *desc;               // batch x cap x 32
     const int32_t *motion_num_valid;   // batch
-    const double *pose_last;           // batch x 16: last_frm.cam_pose_cw_
-    float inv_level_sigma_sq[kMaxLevels];
     const uint8_t *motion_valid;       // batch, may be null (all 1)
     // the reference keyframes (plp_track_keyframe)
     const int32_t *kf_of_frame, *row_offsets;
     const uint8_t *kf_desc;
     const float *kf_angle;
     const uint8_t *kf_valid;           // may be null
-    const double *kf_pos_w;
     const int32_t *fv_offsets;
     const uint32_t *node_ids;
     const int32_t *node_begin;
@@ -64,26 +56,16 @@ struct KfDev {
     uint8_t *claimed;                  // batch x cap
     int32_t *choice, *m21;             // batch x max_kf_points
     BowJob *bjobs;                     // batch
-    PoseJob *posejobs;                 // batch
-    plp_pt_obs *obs;                   // batch x cap
-    int32_t *obs_kp, *obs_row;
-    uint8_t *obs_outlier;
     // outputs
     int32_t *stage, *status;           // batch
     int32_t *matched;                  // batch x cap: matched_lms_in_frm as keyframe rows
     uint32_t *num_bow;                 // batch
-    double *pose;                      // batch x 16
-    int32_t *num_valid, *n_inliers, *lm_iters;  // batch
 };
 
 // the frame runs bow_match_based_track: it needs it and its inputs are in range
 __device__ __forceinline__ bool frame_active(const KfDev &D, int b) {
     return D.stage[b] != 0 && D.status[b] == kStatusOk;
 }
-
-// The kernels have internal linkage, as essential_kernels.cuh's do: robust_track.cu launches the gather and finish
-// kernels as well, over its own matches.
-namespace {
 
 // tracking_module.cc:608-637: the frames the reference hands to bow_match_based_track
 __global__ void __launch_bounds__(kPrepThreads) kf_prep_kernel(KfDev D) {
@@ -208,54 +190,6 @@ __global__ void __launch_bounds__(kThreads) kf_job_kernel(KfDev D) {
         D.bjobs[b] = J;
     }
 }
-
-// frame_tracker.cc:138-163 + pose_optimizer.cc:126-151: below 20 BoW matches the frame fails; otherwise one observation
-// per keypoint holding a keyframe landmark, in keypoint order, and the optimisation starts from last_frm.cam_pose_cw_
-__device__ __forceinline__ bool enough_matches(const KfDev &D, int b) {
-    return frame_active(D, b) && D.num_bow[b] >= (uint32_t)kNumMatchesThr;
-}
-
-__global__ void __launch_bounds__(kThreads) kf_gather_kernel(KfDev D) {
-    const int b = blockIdx.x;
-    const size_t base = (size_t)b * D.cap;
-    const bool enough = enough_matches(D, b);
-    const int r0 = enough ? D.row_offsets[D.kf_of_frame[b]] : 0;
-    const int32_t *matched = D.matched + base;
-    const int n_obs = compact_in_order<kThreads>(
-        enough ? D.n_kp[b] : 0, [&](int i) { return matched[i] >= 0; },
-        [&](int i, int off) {
-            const int q = matched[i];
-            D.obs[base + off] = point_obs(D.kf_pos_w + 3 * (size_t)(r0 + q), D.x[base + i], D.y[base + i],
-                                          D.inv_level_sigma_sq[D.octave[base + i]]);
-            D.obs_kp[base + off] = i;
-            D.obs_row[base + off] = q;
-        });
-    if (threadIdx.x == 0) {  // no observation: the optimiser copies pose_last and reports 0 / 0
-        PoseJob J;
-        J.T_in = D.pose_last + 16 * (size_t)b;
-        J.pts = D.obs + base;
-        J.n_pts = n_obs;
-        J.lines = nullptr;
-        J.n_lines = 0;
-        J.T_out = D.pose + 16 * (size_t)b;
-        J.pt_outlier = D.obs_outlier + base;
-        J.line_outlier = nullptr;
-        J.n_inliers = D.n_inliers + b;
-        J.lm_iters = D.lm_iters + b;
-        D.posejobs[b] = J;
-    }
-}
-
-// frame_tracker::discard_outliers (frame_tracker.cc:166); a frame that failed or did not run keeps no match
-__global__ void __launch_bounds__(kThreads) kf_finish_kernel(KfDev D) {
-    const int b = blockIdx.x;
-    const size_t base = (size_t)b * D.cap;
-    const int valid = discard_outliers<kThreads>(D.n_kp[b], D.posejobs[b].n_pts, enough_matches(D, b),
-                                                 D.obs_outlier + base, D.obs_kp + base, D.matched + base);
-    if (threadIdx.x == 0) D.num_valid[b] = valid;
-}
-
-}  // namespace
 
 }  // namespace kt
 

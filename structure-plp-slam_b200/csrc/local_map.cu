@@ -3,8 +3,9 @@
 //       search_local_landmarks (frame::can_observe + projection::match_frame_and_landmarks, Lowe ratio 0.8)
 //     + pose_optimizer::optimize + the outlier drop and tracked-landmark count
 // for the batch of the tracker's most recent plp_tracker_motion_track_batch_dev, on the same stream and without leaving
-// HBM.  When a plp_tracker_keyframe_track_batch_dev followed that call, its stage-1 frames start from the keyframe track.  It reads that call's inputs, outputs and scratch (tracker.h) and writes separate outputs, so the motion
-// outputs stay as that call wrote them.  Device code: local_map_kernels.cuh.  The window matcher (ratio path) and the
+// HBM.  Each frame starts from the last tracking stage that ran on it: the records of the motion call and of the
+// keyframe and robust calls that followed it (tracker.h).  It reads those calls' inputs, outputs and scratch and writes
+// separate outputs, so theirs stay as they wrote them.  Device code: local_map_kernels.cuh.  The window matcher (ratio path) and the
 // pose optimiser are the existing launchers, and the predict_scale_level table is plp_fuse_level_thresholds'.
 //
 // This file is compiled with -fmad=false (build.py FILE_FLAGS): can_observe's double / float mix rounds like the oracle.
@@ -95,11 +96,11 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
                 "local-map arrays");
     PLP_REQUIRE(t->d_local, "plp_tracker_reserve_local_map has not been called");
     PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
-    PLP_REQUIRE(t->has_motion && batch <= t->motion.batch,
+    PLP_REQUIRE(t->covers(kStageMotion, batch),
                 "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
-    PLP_REQUIRE(!t->has_kf || batch <= t->kf_batch,
+    PLP_REQUIRE(!t->record_batch[kStageKeyframe] || t->covers(kStageKeyframe, batch),
                 "the batch must not exceed that of the plp_tracker_keyframe_track_batch_dev that followed the motion track");
-    PLP_REQUIRE(!t->has_rb || batch <= t->rb_batch,
+    PLP_REQUIRE(!t->record_batch[kStageRobust] || t->covers(kStageRobust, batch),
                 "the batch must not exceed that of the plp_tracker_robust_track_batch_dev that followed the keyframe track");
     PLP_REQUIRE(margin > 0.0f, "margin");
     plp_ctx *ctx = t->ctx;
@@ -112,16 +113,12 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.y = M.y;
     D.octave = M.octave;
     D.desc = M.desc;
-    D.last_pos_w = M.last_pos_w;
-    D.last_offsets = M.last_offsets;
-    D.motion_matched = M.matched;
-    D.motion_pose = M.pose_out;
-    D.motion_num_valid = M.num_valid;
-    D.motion_jobs = M.posejobs;
-    D.obs_last = M.obs_last;
-    for (int l = 0; l < 16; ++l) D.inv_level_sigma_sq[l] = M.inv_level_sigma_sq[l];
-    if (t->has_kf) D.kf = t->kf_track;  // else D.kf.stage stays null: every frame starts from its motion track
-    if (t->has_rb) D.rb = t->rb_track;  // else D.rb.stage stays null: no frame starts from a robust track
+    for (int l = 0; l < 16; ++l) D.inv_level_sigma_sq[l] = t->tail[kStageMotion].inv_level_sigma_sq[l];
+    D.motion = t->record[kStageMotion];
+    D.motion.local_idx = local->last_local_idx;  // one entry per last-frame row
+    D.motion.local_idx_offsets = M.last_offsets;
+    if (t->record_batch[kStageKeyframe]) D.kf = t->record[kStageKeyframe];  // else D.kf.stage stays null
+    if (t->record_batch[kStageRobust]) D.rb = t->record[kStageRobust];      // else D.rb.stage stays null
     D.pos_w = local->pos_w;
     D.normal = local->obs_mean_normal;
     D.min_d = local->min_valid_dist;
@@ -130,7 +127,6 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.lm_desc = local->desc;
     D.valid = local->valid;
     D.offsets = local->offsets;
-    D.last_local_idx = local->last_local_idx;
     D.margin = margin;
     D.matched = d_matched_out;
     D.local = d_local_out;
@@ -152,7 +148,7 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     PLP_LAUNCH(ctx, local_gather_kernel, batch, lm::kThreads, 0, D);
     PLP_CHECK_LAUNCH();
     plp_pose_opt_cfg cfg{4, 10};
-    PLP_TRY(launch_pose_opt(ctx, D.posejobs, batch, t->cap, t->cam, cfg));
+    PLP_TRY(launch_pose_opt(ctx, D.posejobs, batch, t->cam, cfg));
     PLP_LAUNCH(ctx, local_finish_kernel, batch, lm::kThreads, 0, D);
     PLP_CHECK_LAUNCH();
     return PLP_OK;

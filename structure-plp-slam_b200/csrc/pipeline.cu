@@ -24,8 +24,6 @@ namespace plp {
 
 namespace {
 
-constexpr int kNumMatchesThr = 20;  // frame_tracker::num_matches_thr_ (module/frame_tracker.h)
-
 __global__ void track_prep_kernel(TrackDev T, float margin, int check_orientation) {
     const int b = blockIdx.x, tid = threadIdx.x;
     const int n = T.n_kp[b];
@@ -97,49 +95,17 @@ __global__ void track_retry_gate_kernel(TrackDev T) {
     }
 }
 
-// 2D-3D observations of the matched keypoints, in keypoint order (pose_optimizer.cc:126-151)
-__global__ void track_gather_kernel(TrackDev T) {
-    const int b = blockIdx.x, tid = threadIdx.x;
-    const size_t base = (size_t)b * T.cap;
-    const int l0 = T.last_offsets[b];
-    const bool enough = T.num_matches[b] >= (uint32_t)kNumMatchesThr;  // frame_tracker.cc:73-77
-    const int32_t *matched = T.matched + base;
-    const int n_obs = compact_in_order<256>(
-        T.n_kp[b], [&](int i) { return enough && matched[i] >= 0; },
-        [&](int i, int off) {
-            const int q = matched[i];
-            T.obs[base + off] = point_obs(T.last_pos_w + 3 * (size_t)(l0 + q), T.x[base + i], T.y[base + i],
-                                          T.inv_level_sigma_sq[T.octave[base + i]]);
-            T.obs_kp[base + off] = i;
-            T.obs_last[base + off] = q;
-        });
-    if (tid == 0) {
-        PoseJob J;
-        J.T_in = T.pose_pred + 16 * (size_t)b;
-        J.pts = T.obs + base;
-        J.n_pts = n_obs;
-        J.lines = nullptr;
-        J.n_lines = 0;
-        J.T_out = T.pose_out + 16 * (size_t)b;
-        J.pt_outlier = T.obs_outlier + base;
-        J.line_outlier = nullptr;
-        J.n_inliers = T.n_inliers + b;
-        J.lm_iters = T.lm_iters + b;
-        T.posejobs[b] = J;
-    }
-}
-
-// frame_tracker::discard_outliers (frame_tracker.cc:253-283)
-__global__ void track_finish_kernel(TrackDev T) {
-    const int b = blockIdx.x;
-    const size_t base = (size_t)b * T.cap;
-    const bool enough = T.num_matches[b] >= (uint32_t)kNumMatchesThr;
-    const int valid = discard_outliers<256>(T.n_kp[b], T.posejobs[b].n_pts, enough, T.obs_outlier + base,
-                                            T.obs_kp + base, T.matched + base);
-    if (threadIdx.x == 0) T.num_valid[b] = valid;
-}
-
 }  // namespace
+
+plp_status launch_track_tail(plp_ctx *ctx, const TrackTail &J, int batch, const plp_camera &cam) {
+    PLP_LAUNCH(ctx, track_gather_kernel, batch, kTailThreads, 0, J);
+    PLP_CHECK_LAUNCH();
+    plp_pose_opt_cfg cfg{4, 10};
+    PLP_TRY(launch_pose_opt(ctx, J.posejobs, batch, cam, cfg));
+    PLP_LAUNCH(ctx, track_finish_kernel, batch, kTailThreads, 0, J);
+    PLP_CHECK_LAUNCH();
+    return PLP_OK;
+}
 
 }  // namespace plp
 
@@ -206,12 +172,15 @@ plp_status plp_tracker_create_ex(plp_ctx *ctx, const plp_camera *cam, const plp_
     L.out(T.num_matches, B);
     L.out(T.pjobs, 2 * B);
     L.out(T.mjobs, 2 * B);
-    L.out(T.posejobs, B);
-    L.out(T.obs, B * C);
-    L.out(T.obs_kp, B * C);
-    L.out(T.obs_outlier, B * C);
-    L.out(T.obs_last, B * C);
-    for (int l = 0; l < 16; ++l) T.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
+    TrackTail &J = t->tail[kStageMotion];
+    memset(&J, 0, sizeof(J));
+    J.cap = kp_capacity;
+    for (int l = 0; l < 16; ++l) J.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
+    L.out(J.posejobs, B);
+    L.out(J.obs, B * C);
+    L.out(J.obs_kp, B * C);
+    L.out(J.obs_outlier, B * C);
+    L.out(J.obs_row, B * C);
     if (distorted) {
         t->distorted = true;
         t->undist = uj;
@@ -264,9 +233,7 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
                     last->pose_last,
                 "last-frame arrays");
     plp_ctx *ctx = t->ctx;
-    t->has_motion = false;
-    t->has_kf = false;
-    t->has_rb = false;
+    t->invalidate_from(kStageMotion);
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     TrackDev T = t->dev;
     T.batch = batch;
@@ -282,10 +249,6 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
     T.pose_pred = last->pose_pred;
     T.pose_last = last->pose_last;
     T.matched = d_matched_out;
-    T.pose_out = d_pose_out;
-    T.num_valid = d_num_valid_out;
-    T.n_inliers = d_n_inliers_out;
-    T.lm_iters = d_lm_iters_out;
     if (t->distorted) {  // frame.cc:68,79: undist_keypts_ and bearings_ of the current frames
         UndistJob J = t->undist;
         J.batch = batch;
@@ -309,14 +272,23 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
                                   2 * margin));
     PLP_TRY(launch_point_match(ctx, T.mjobs + batch, batch, t->cap > kMatchMaxPoints ? kMatchMaxPoints : t->cap, t->grid,
                                0, 0.0f, 1));
-    PLP_LAUNCH(ctx, track_gather_kernel, batch, 256, 0, T);
-    PLP_CHECK_LAUNCH();
-    plp_pose_opt_cfg cfg{4, 10};
-    PLP_TRY(launch_pose_opt(ctx, T.posejobs, batch, t->cap > 6144 ? 6144 : t->cap, t->cam, cfg));
-    PLP_LAUNCH(ctx, track_finish_kernel, batch, 256, 0, T);
-    PLP_CHECK_LAUNCH();
+    // pose-opt from the predicted pose over the frames with 20 matches (frame_tracker.cc:73-108)
+    TrackTail J = t->tail[kStageMotion];
+    J.n_kp = d_n_kp;
+    J.x = T.x;
+    J.y = T.y;
+    J.octave = T.octave;
+    J.count = (const int32_t *)T.num_matches;  // the matcher's count (uint32_t), far below 2^31
+    J.rows = TrackRows{T.last_pos_w, T.last_offsets, nullptr};
+    J.pose_in = T.pose_pred;
+    J.matched = d_matched_out;
+    J.pose = d_pose_out;
+    J.num_valid = d_num_valid_out;
+    J.n_inliers = d_n_inliers_out;
+    J.lm_iters = d_lm_iters_out;
+    PLP_TRY(launch_track_tail(ctx, J, batch, t->cam));
     t->motion = T;
-    t->has_motion = true;
+    t->set_record(kStageMotion, batch, J, nullptr, nullptr);  // local_map.cu binds last_local_idx
     return PLP_OK;
 }
 

@@ -6,7 +6,7 @@
 
 namespace plp {
 
-plp_status launch_pose_opt(plp_ctx *ctx, const PoseJob *d_jobs, int batch, int max_edges, const plp_camera &cam,
+plp_status launch_pose_opt(plp_ctx *ctx, const PoseJob *d_jobs, int batch, const plp_camera &cam,
                            const plp_pose_opt_cfg &cfg);
 
 }  // namespace plp

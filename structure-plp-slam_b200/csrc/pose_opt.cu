@@ -49,9 +49,8 @@ __global__ void build_pose_jobs_kernel(PoseJob *jobs, int batch, const double *T
 
 }  // namespace
 
-plp_status launch_pose_opt(plp_ctx *ctx, const PoseJob *d_jobs, int batch, int max_edges, const plp_camera &cam,
+plp_status launch_pose_opt(plp_ctx *ctx, const PoseJob *d_jobs, int batch, const plp_camera &cam,
                            const plp_pose_opt_cfg &cfg) {
-    (void)max_edges;  // no per-frame shared-memory tables any more: the edge count is unbounded
     if (batch <= 0) return PLP_OK;
     using po::pose_opt_kernel;
     PLP_LAUNCH(ctx, pose_opt_kernel, batch, po::kThreads, 0, d_jobs, batch, cam, cfg);
@@ -81,7 +80,8 @@ plp_status plp_pose_optimize_batch_dev(plp_ctx *ctx, const plp_camera *cam, int 
     PLP_LAUNCH(ctx, build_pose_jobs_kernel, div_up(batch, 128), 128, 0, (PoseJob *)d_jobs, batch, d_T_in, d_pts,
                d_pt_off, d_lines, d_line_off, d_T_out, d_pt_outlier, d_line_outlier, d_n_inliers, d_lm_iters);
     PLP_CHECK_LAUNCH();
-    return launch_pose_opt(ctx, (const PoseJob *)d_jobs, batch, max_edges_per_frame, *cam, *cfg);
+    (void)max_edges_per_frame;  // no per-frame shared-memory tables any more: the edge count is unbounded
+    return launch_pose_opt(ctx, (const PoseJob *)d_jobs, batch, *cam, *cfg);
 }
 
 plp_status plp_pose_optimize_batch(plp_ctx *ctx, const plp_camera *cam, int batch, const double *T_in,

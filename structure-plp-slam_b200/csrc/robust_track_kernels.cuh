@@ -6,8 +6,7 @@
 //   -> below 20 the frame fails; else pose_optimizer::optimize from last_frm.cam_pose_cw_ -> discard_outliers.
 // Free of host-side CUDA runtime dependencies so that tests/cta_emu can compile the same text for the host.
 //
-// Kernels, in launch order (brute_match_kernel, kt::kf_gather_kernel, the pose optimiser and kt::kf_finish_kernel in
-// between and after are the existing ones):
+// Kernels, in launch order (brute_match_kernel in between is the existing one):
 //   rt_prep_kernel        one thread per frame: stage flag, status, the BruteJob (empty for a frame that does not run)
 //   rt_list_kernel        one CTA per frame: the brute-force match list in frame keypoint order, the frame's bearings
 //                         (undistorted tracker), the 50 x 8 sample sets (ransac_sample.h)
@@ -15,6 +14,7 @@
 //                         are staged in shared memory, only E and the score are kept
 //   rt_select_kernel      one CTA per frame: the first-best replay, validity, the winner's inlier flags (recomputed)
 //                         and the robust matches
+// then the tail of track_common.cuh: count = the robust matches, rows = the keyframes', from last_frm.cam_pose_cw_.
 #pragma once
 #include <stddef.h>
 #include <stdint.h>
@@ -24,7 +24,6 @@
 #include "devmath.cuh"
 #include "essential_common.cuh"
 #include "match_jobs.h"
-#include "pose_jobs.h"
 #include "ransac_sample.h"
 #include "track_common.cuh"
 
@@ -35,7 +34,6 @@ namespace rt {
 constexpr int kThreads = 256;         // list: one CTA per frame
 constexpr int kEssThreads = 128;      // hypothesis / select
 constexpr int kPrepThreads = 128;
-constexpr int kNumMatchesThr = 20;    // frame_tracker::num_matches_thr_
 constexpr float kLoweRatio = 0.8f;    // frame_tracker.cc:196: robust robust_matcher(0.8, false)
 constexpr int kNumIter = 50;          // robust.cc:233: find_via_ransac(50, false)
 constexpr int kMinSet = 8;            // essential_solver.cc:44
@@ -68,11 +66,6 @@ struct RtDev {
     uint8_t *inlier;                   // batch x cap: the winner's flag per match-list entry
     double *best_score;                // batch
     int32_t *valid;                    // batch: solution_is_valid_
-    // scratch of the gather, the pose optimisation and discard_outliers (kt::kf_gather_kernel, kt::kf_finish_kernel)
-    PoseJob *posejobs;                 // batch
-    plp_pt_obs *obs;                   // batch x cap
-    int32_t *obs_kp, *obs_row;
-    uint8_t *obs_outlier;
     // outputs
     int32_t *stage, *status;           // batch
     int32_t *matched;                  // batch x cap: brute-force matches, then the robust ones (keyframe rows)

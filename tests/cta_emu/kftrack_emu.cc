@@ -1,8 +1,9 @@
 // kftrack_emu.cc -- csrc/keyframe_track_kernels.cuh (the batched keyframe tracker) executed on the host, with
-// bow_match_kernel (bow_kernels.cuh) between the job and gather kernels.  The pose optimiser is not emulated:
-// emu_kf_begin runs prep -> transform -> job -> bow match -> gather and returns what they wrote; the caller optimises
-// the gathered observations and hands the outlier flags to emu_kf_finish.  With node_desc == nullptr the transform is
-// skipped and the caller's word / node / weight rows stand for it, so that a test can pick the feature vectors.
+// bow_match_kernel (bow_kernels.cuh) between the job kernel and the tail (track_common.cuh).  The pose optimiser is not
+// emulated: emu_kf_begin runs prep -> transform -> job -> bow match -> gather and returns what they wrote; the caller
+// optimises the gathered observations and hands the outlier flags to emu_tail_finish.  With node_desc == nullptr the
+// transform is skipped and the caller's word / node / weight rows stand for it, so that a test can pick the feature
+// vectors.  emu_tail_begin runs the gather alone, for a tail job of the caller's (e.g. the motion stage's form).
 #include "cta_emu.h"
 
 #include <string.h>
@@ -16,11 +17,53 @@ using namespace plp;
 namespace {
 
 kt::KfDev g_D;
-std::vector<int32_t> g_nb1, g_ne1, g_nb2, g_ne2, g_choice, g_m21, g_n_inl, g_iters, g_obs_kp;
+TrackTail g_J;
+std::vector<int32_t> g_nb1, g_ne1, g_nb2, g_ne2, g_choice, g_m21, g_n_inl, g_iters;
 std::vector<uint8_t> g_claimed, g_outlier;
 std::vector<BowJob> g_bjobs;
 std::vector<PoseJob> g_posejobs;
 std::vector<double> g_pose;
+
+// the tail job over the caller's keypoints, gate, rows and observation outputs, with the scratch above
+void bind_tail(int batch, int cap, const int32_t *n_kp, const float *x, const float *y, const int32_t *octave,
+               const float *inv_level_sigma_sq, int num_levels, const int32_t *count, const int32_t *stage,
+               const int32_t *status, TrackRows rows, const double *pose_in, int32_t *matched, plp_pt_obs *obs,
+               int32_t *obs_kp, int32_t *obs_row) {
+    const size_t B = batch, C = cap;
+    g_outlier.assign(B * C, 0);
+    g_posejobs.assign(B, PoseJob{});
+    g_pose.assign(B * 16, 0.0);
+    g_n_inl.assign(B, 0);
+    g_iters.assign(B, 0);
+    TrackTail &J = g_J;
+    memset(&J, 0, sizeof(J));
+    J.cap = cap;
+    J.n_kp = n_kp;
+    J.x = x;
+    J.y = y;
+    J.octave = octave;
+    for (int l = 0; l < 16; ++l) J.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
+    J.count = count;
+    J.stage = stage;
+    J.status = status;
+    J.rows = rows;
+    J.pose_in = pose_in;
+    J.matched = matched;
+    J.posejobs = g_posejobs.data();
+    J.obs = obs;
+    J.obs_kp = obs_kp;
+    J.obs_row = obs_row;
+    J.obs_outlier = g_outlier.data();
+    J.pose = g_pose.data();
+    J.num_valid = nullptr;  // set by emu_tail_finish
+    J.n_inliers = g_n_inl.data();
+    J.lm_iters = g_iters.data();
+}
+
+void tail_gather(int batch, int32_t *n_obs) {
+    emu_launch(track_gather_kernel, (unsigned)batch, (unsigned)kTailThreads, g_J);
+    for (int b = 0; b < batch; ++b) n_obs[b] = g_posejobs[b].n_pts;
+}
 
 }  // namespace
 
@@ -44,13 +87,8 @@ extern "C" void emu_kf_begin(int batch, int cap, int num_keyframes, int max_kf_p
     g_ne2.assign(B * C, -7);
     g_choice.assign(B * R, 0);
     g_m21.assign(B * R, 0);
-    g_n_inl.assign(B, 0);
-    g_iters.assign(B, 0);
     g_claimed.assign(B * C, 1);
-    g_outlier.assign(B * C, 0);
     g_bjobs.assign(B, BowJob{});
-    g_posejobs.assign(B, PoseJob{});
-    g_pose.assign(B * 16, 0.0);
     kt::KfDev &D = g_D;
     memset(&D, 0, sizeof(D));
     D.batch = batch;
@@ -58,21 +96,15 @@ extern "C" void emu_kf_begin(int batch, int cap, int num_keyframes, int max_kf_p
     D.num_keyframes = num_keyframes;
     D.max_kf_points = max_kf_points;
     D.n_kp = n_kp;
-    D.x = x;
-    D.y = y;
     D.angle = angle;
-    D.octave = octave;
     D.desc = desc;
     D.motion_num_valid = motion_num_valid;
-    D.pose_last = pose_last;
-    for (int l = 0; l < kt::kMaxLevels; ++l) D.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
     D.motion_valid = motion_valid;
     D.kf_of_frame = kf_of_frame;
     D.row_offsets = row_offsets;
     D.kf_desc = kf_desc;
     D.kf_angle = kf_angle;
     D.kf_valid = kf_valid;
-    D.kf_pos_w = kf_pos_w;
     D.fv_offsets = fv_offsets;
     D.node_ids = node_ids;
     D.node_begin = node_begin;
@@ -89,19 +121,12 @@ extern "C" void emu_kf_begin(int batch, int cap, int num_keyframes, int max_kf_p
     D.choice = g_choice.data();
     D.m21 = g_m21.data();
     D.bjobs = g_bjobs.data();
-    D.posejobs = g_posejobs.data();
-    D.obs = obs;
-    D.obs_kp = obs_kp;
-    D.obs_row = obs_row;
-    D.obs_outlier = g_outlier.data();
     D.stage = stage;
     D.status = status;
     D.matched = matched;
     D.num_bow = num_bow;
-    D.pose = g_pose.data();
-    D.num_valid = nullptr;  // set by emu_kf_finish
-    D.n_inliers = g_n_inl.data();
-    D.lm_iters = g_iters.data();
+    bind_tail(batch, cap, n_kp, x, y, octave, inv_level_sigma_sq, num_levels, (const int32_t *)num_bow, stage, status,
+              TrackRows{kf_pos_w, row_offsets, kf_of_frame}, pose_last, matched, obs, obs_kp, obs_row);
 
     emu_launch(kt::kf_prep_kernel, (unsigned)((batch + kt::kPrepThreads - 1) / kt::kPrepThreads),
                (unsigned)kt::kPrepThreads, D);
@@ -127,12 +152,24 @@ extern "C" void emu_kf_begin(int batch, int cap, int num_keyframes, int max_kf_p
     memcpy(ne2, g_ne2.data(), B * C * 4);
     emu_launch(bow_match_kernel, (unsigned)batch, (unsigned)kMatchThreads, (const BowJob *)g_bjobs.data(),
                kt::kLoweRatio, 1);
-    emu_launch(kt::kf_gather_kernel, (unsigned)batch, (unsigned)kt::kThreads, D);
-    for (size_t b = 0; b < B; ++b) n_obs[b] = g_posejobs[b].n_pts;
+    tail_gather(batch, n_obs);
 }
 
-extern "C" void emu_kf_finish(const uint8_t *outlier, int32_t *num_valid) {
+// the gather of a tail job whose gate is `count` alone where stage / status are null; t_in[b]: the frame whose pose_in
+// row the pose job starts from
+extern "C" void emu_tail_begin(int batch, int cap, const int32_t *n_kp, const float *x, const float *y,
+                               const int32_t *octave, const float *inv_level_sigma_sq, int num_levels,
+                               const int32_t *count, const int32_t *stage, const int32_t *status, const double *pos_w,
+                               const int32_t *offsets, const int32_t *of_frame, const double *pose_in, int32_t *matched,
+                               plp_pt_obs *obs, int32_t *obs_kp, int32_t *obs_row, int32_t *n_obs, int32_t *t_in) {
+    bind_tail(batch, cap, n_kp, x, y, octave, inv_level_sigma_sq, num_levels, count, stage, status,
+              TrackRows{pos_w, offsets, of_frame}, pose_in, matched, obs, obs_kp, obs_row);
+    tail_gather(batch, n_obs);
+    for (int b = 0; b < batch; ++b) t_in[b] = (int32_t)((g_posejobs[b].T_in - pose_in) / 16);
+}
+
+extern "C" void emu_tail_finish(const uint8_t *outlier, int32_t *num_valid) {
     memcpy(g_outlier.data(), outlier, g_outlier.size());
-    g_D.num_valid = num_valid;
-    emu_launch(kt::kf_finish_kernel, (unsigned)g_D.batch, (unsigned)kt::kThreads, g_D);
+    g_J.num_valid = num_valid;
+    emu_launch(track_finish_kernel, (unsigned)g_posejobs.size(), (unsigned)kTailThreads, g_J);
 }

@@ -1,7 +1,7 @@
 // local_map_emu.cc -- csrc/local_map_kernels.cuh (the local-map stage of tracking) executed on the host, with the window
 // matcher of point_match_kernels.cuh between observe and gather.  The pose optimiser is not emulated: emu_local_begin
 // runs prep -> observe -> match -> gather and returns the gathered observations; the caller optimises them and hands
-// the outlier flags to emu_local_finish.
+// the outlier flags to emu_local_finish.  The motion, keyframe and robust records come as EmuRecords.
 #include "cta_emu.h"
 
 #include <string.h>
@@ -22,17 +22,27 @@ std::vector<float> g_qx, g_qy, g_qr;
 std::vector<int32_t> g_qmin, g_qmax, g_choice, g_best, g_obs_kp, g_n_inl, g_iters;
 std::vector<uint32_t> g_nm;
 std::vector<PointMatchJob> g_mjobs;
-std::vector<PoseJob> g_motion_jobs, g_posejobs;
+std::vector<PoseJob> g_posejobs, g_record_jobs[3];
 std::vector<plp_pt_obs> g_obs;
 std::vector<double> g_pose;
 
 }  // namespace
 
+// one TrackRecord as the caller's arrays, n_obs[b] standing for posejobs[b].n_pts; a keyframe or robust record with
+// stage == nullptr is left out
+struct EmuRecord {
+    const int32_t *stage, *status, *matched;
+    const double *pose;
+    const int32_t *num_valid, *n_obs, *obs_row;
+    const double *pos_w;
+    const int32_t *offsets, *of_frame, *local_idx, *local_idx_offsets;
+};
+
+// records: motion, keyframe, robust.  As local_map.cu does, the motion record's local_idx is last_local_idx over its
+// row offsets.
 extern "C" void emu_local_begin(const plp_grid *grid, const plp_camera *cam, int batch, int cap, int max_local,
                                 const int32_t *n_kp, const float *x, const float *y, const int32_t *octave,
-                                const uint8_t *desc, const double *last_pos_w, const int32_t *last_offsets,
-                                const int32_t *motion_matched, const double *motion_pose, const int32_t *motion_num_valid,
-                                const int32_t *n_obs1, const int32_t *obs_last, const float *inv_level_sigma_sq,
+                                const uint8_t *desc, const EmuRecord *records, const float *inv_level_sigma_sq,
                                 const double *pos_w, const double *normal, const float *min_d, const float *max_d,
                                 const float *max_raw, const uint8_t *lm_desc, const uint8_t *valid,
                                 const int32_t *offsets, const int32_t *last_local_idx, const float *scale_factors,
@@ -59,11 +69,20 @@ extern "C" void emu_local_begin(const plp_grid *grid, const plp_camera *cam, int
     g_iters.assign(B, 0);
     g_nm.assign(B, 0);
     g_mjobs.assign(B, PointMatchJob{});
-    g_motion_jobs.assign(B, PoseJob{});
     g_posejobs.assign(B, PoseJob{});
     g_obs.assign(B * C, plp_pt_obs{});
     g_pose.assign(B * 16, 0.0);
-    for (size_t b = 0; b < B; ++b) g_motion_jobs[b].n_pts = n_obs1[b];
+    TrackRecord rec[3] = {};
+    for (int s = 0; s < 3; ++s) {
+        const EmuRecord &E = records[s];
+        if (s > 0 && !E.stage) continue;
+        g_record_jobs[s].assign(B, PoseJob{});
+        for (size_t b = 0; b < B; ++b) g_record_jobs[s][b].n_pts = E.n_obs[b];
+        rec[s] = TrackRecord{E.stage,    E.status,     E.matched, E.pose,         E.num_valid, g_record_jobs[s].data(),
+                             E.obs_row, TrackRows{E.pos_w, E.offsets, E.of_frame}, E.local_idx, E.local_idx_offsets};
+    }
+    rec[0].local_idx = last_local_idx;
+    rec[0].local_idx_offsets = records[0].offsets;
     lm::LocalDev &D = g_D;
     memset(&D, 0, sizeof(D));
     D.batch = batch;
@@ -74,13 +93,9 @@ extern "C" void emu_local_begin(const plp_grid *grid, const plp_camera *cam, int
     D.y = y;
     D.octave = octave;
     D.desc = desc;
-    D.last_pos_w = last_pos_w;
-    D.last_offsets = last_offsets;
-    D.motion_matched = motion_matched;
-    D.motion_pose = motion_pose;
-    D.motion_num_valid = motion_num_valid;
-    D.motion_jobs = g_motion_jobs.data();
-    D.obs_last = obs_last;
+    D.motion = rec[0];
+    D.kf = rec[1];
+    D.rb = rec[2];
     for (int l = 0; l < lm::kMaxLevels; ++l) {
         D.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
         D.scale_factors[l] = l < num_levels ? scale_factors[l] : 1.0f;
@@ -94,7 +109,6 @@ extern "C" void emu_local_begin(const plp_grid *grid, const plp_camera *cam, int
     D.lm_desc = lm_desc;
     D.valid = valid;
     D.offsets = offsets;
-    D.last_local_idx = last_local_idx;
     D.cam = *cam;
     D.num_levels = num_levels;
     D.margin = margin;

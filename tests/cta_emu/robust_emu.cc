@@ -1,5 +1,5 @@
-// robust_emu.cc -- csrc/robust_track_kernels.cuh (the batched robust tracker) executed on the host, with the keyframe
-// tracker's gather and finish kernels (keyframe_track_kernels.cuh) after it.  Neither the brute-force matcher nor the
+// robust_emu.cc -- csrc/robust_track_kernels.cuh (the batched robust tracker) executed on the host, with the tail
+// (track_common.cuh) after it.  Neither the brute-force matcher nor the
 // pose optimiser is emulated: the caller hands in the brute-force matches of every frame (as brute_match_kernel leaves
 // them in matched_out), emu_rt_begin runs prep -> list -> hypotheses -> select -> gather and returns what they wrote,
 // and the caller hands the optimiser's outlier flags to emu_rt_finish.
@@ -9,7 +9,6 @@
 
 #include <vector>
 
-#include "keyframe_track_kernels.cuh"
 #include "robust_track_kernels.cuh"
 
 using namespace plp;
@@ -17,7 +16,7 @@ using namespace plp;
 namespace {
 
 rt::RtDev g_D;
-kt::KfDev g_G;
+TrackTail g_J;
 std::vector<BruteJob> g_bjobs;
 std::vector<PoseJob> g_posejobs;
 std::vector<uint8_t> g_outlier;
@@ -101,11 +100,6 @@ extern "C" void emu_rt_begin(int batch, int cap, uint64_t seed, const int32_t *n
     D.inlier = inlier;
     D.best_score = best_score;
     D.valid = valid;
-    D.posejobs = g_posejobs.data();
-    D.obs = obs;
-    D.obs_kp = obs_kp;
-    D.obs_row = obs_row;
-    D.obs_outlier = g_outlier.data();
     D.stage = stage;
     D.status = status;
     D.matched = matched;
@@ -122,37 +116,34 @@ extern "C" void emu_rt_begin(int batch, int cap, uint64_t seed, const int32_t *n
                 (size_t)cap * 2 * sizeof(float), D);
     emu_launch(rt::rt_select_kernel, (unsigned)batch, (unsigned)rt::kEssThreads, D);
 
-    kt::KfDev &G = g_G;
-    memset(&G, 0, sizeof(G));
-    G.batch = batch;
-    G.cap = cap;
-    G.n_kp = n_kp;
-    G.x = x;
-    G.y = y;
-    G.octave = octave;
-    G.pose_last = pose_last;
-    for (int l = 0; l < kt::kMaxLevels; ++l) G.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
-    G.kf_of_frame = kf_of_frame;
-    G.row_offsets = row_offsets;
-    G.kf_pos_w = kf_pos_w;
-    G.posejobs = g_posejobs.data();
-    G.obs = obs;
-    G.obs_kp = obs_kp;
-    G.obs_row = obs_row;
-    G.obs_outlier = g_outlier.data();
-    G.stage = stage;
-    G.status = status;
-    G.matched = matched;
-    G.num_bow = (uint32_t *)num_robust;
-    G.pose = g_pose.data();
-    G.n_inliers = g_n_inl.data();
-    G.lm_iters = g_iters.data();
-    emu_launch(kt::kf_gather_kernel, (unsigned)batch, (unsigned)kt::kThreads, G);
+    TrackTail &J = g_J;
+    memset(&J, 0, sizeof(J));
+    J.cap = cap;
+    J.n_kp = n_kp;
+    J.x = x;
+    J.y = y;
+    J.octave = octave;
+    for (int l = 0; l < 16; ++l) J.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
+    J.count = num_robust;
+    J.stage = stage;
+    J.status = status;
+    J.rows = TrackRows{kf_pos_w, row_offsets, kf_of_frame};
+    J.pose_in = pose_last;
+    J.matched = matched;
+    J.posejobs = g_posejobs.data();
+    J.obs = obs;
+    J.obs_kp = obs_kp;
+    J.obs_row = obs_row;
+    J.obs_outlier = g_outlier.data();
+    J.pose = g_pose.data();
+    J.n_inliers = g_n_inl.data();
+    J.lm_iters = g_iters.data();
+    emu_launch(track_gather_kernel, (unsigned)batch, (unsigned)kTailThreads, J);
     for (size_t b = 0; b < B; ++b) n_obs[b] = g_posejobs[b].n_pts;
 }
 
 extern "C" void emu_rt_finish(const uint8_t *outlier, int32_t *num_valid) {
     memcpy(g_outlier.data(), outlier, g_outlier.size());
-    g_G.num_valid = num_valid;
-    emu_launch(kt::kf_finish_kernel, (unsigned)g_G.batch, (unsigned)kt::kThreads, g_G);
+    g_J.num_valid = num_valid;
+    emu_launch(track_finish_kernel, (unsigned)g_D.batch, (unsigned)kTailThreads, g_J);
 }

@@ -138,7 +138,7 @@ def _run(emu, plp, frames, kfs, kf_of_frame, motion_num_valid, motion_valid, max
     # the pose optimiser is not emulated: random outlier flags stand for its result
     outlier = (rng.random((B, cap)) < 0.2).astype(np.uint8)
     num_valid = np.full(B, -3, np.int32)
-    emu.emu_kf_finish(_ptr(outlier), _ptr(num_valid))
+    emu.emu_tail_finish(_ptr(outlier), _ptr(num_valid))
     got.update(matched=matched, num_valid=num_valid, outlier=outlier)
     return got
 
@@ -189,20 +189,27 @@ def _expect_and_compare(orc, plp, got, frames, kfs, kf_of_frame, motion_num_vali
         _, m12, num = orc.bow_tree_match(side1, side2, 0.7, True)
         assert got["num_bow"][b] == num, (b, got["num_bow"][b], num)
         assert np.array_equal(got["matched_pre"][b, :n], m12), b
-        if num < 20:
-            assert got["n_obs"][b] == 0 and (got["matched"][b, :n] == -1).all() and got["num_valid"][b] == 0, b
-            continue
-        sel = np.nonzero(m12 >= 0)[0]
-        no = len(sel)
-        assert got["n_obs"][b] == no, b
-        assert np.array_equal(got["obs_kp"][b, :no], sel) and np.array_equal(got["obs_row"][b, :no], m12[sel]), b
-        o = got["obs"][b, :no]
-        assert np.array_equal(o["pos_w"], kfs[k]["pos_w"][m12[sel]]), b
-        assert np.array_equal(o["obs_x"], f["x"][sel]) and np.array_equal(o["obs_y"], f["y"][sel]), b
-        assert (o["x_right"] == -1.0).all() and np.array_equal(o["inv_sigma_sq"], ISIG[f["octave"][sel]]), b
-        post = m12.copy()
-        post[sel[got["outlier"][b, :no] != 0]] = -1
-        assert np.array_equal(got["matched"][b, :n], post) and got["num_valid"][b] == (post >= 0).sum(), b
+        _expect_tail(got, b, num, m12, kfs[k]["pos_w"], f)
+
+
+def _expect_tail(got, b, count, m12, pos_w, f):
+    """The tail (track_common.cuh) of frame b: below 20 matches nothing is gathered and every match is dropped;
+    otherwise one observation per matched keypoint in keypoint order (its row's pos_w), then discard_outliers."""
+    n = len(f["x"])
+    if count < 20:
+        assert got["n_obs"][b] == 0 and (got["matched"][b, :n] == -1).all() and got["num_valid"][b] == 0, b
+        return
+    sel = np.nonzero(m12 >= 0)[0]
+    no = len(sel)
+    assert got["n_obs"][b] == no, b
+    assert np.array_equal(got["obs_kp"][b, :no], sel) and np.array_equal(got["obs_row"][b, :no], m12[sel]), b
+    o = got["obs"][b, :no]
+    assert np.array_equal(o["pos_w"], pos_w[m12[sel]]), b
+    assert np.array_equal(o["obs_x"], f["x"][sel]) and np.array_equal(o["obs_y"], f["y"][sel]), b
+    assert (o["x_right"] == -1.0).all() and np.array_equal(o["inv_sigma_sq"], ISIG[f["octave"][sel]]), b
+    post = m12.copy()
+    post[sel[got["outlier"][b, :no] != 0]] = -1
+    assert np.array_equal(got["matched"][b, :n], post) and got["num_valid"][b] == (post >= 0).sum(), b
 
 
 def test_keyframe_track_kernels_on_cpu_equal_restatement(emu, orc, plp):
@@ -274,3 +281,44 @@ def test_keyframe_track_transform_runs_on_active_frames_only(emu, orc, plp):
         assert list(got["stage"]) == [1, 0, 1]
     finally:
         orc.bow_vocab_destroy(ov)
+
+
+def test_track_tail_motion_form_on_cpu_equal_restatement(emu):
+    """The shared tail with null stage / status, as the motion stage binds it: the gate is the match count alone, frame
+    b's rows are block b of the last frames' rows, and the optimisation starts from frame b's predicted pose."""
+    rng = np.random.default_rng(63)
+    counts = [57, 19, 20, 0, 300, 21]
+    B, cap = len(counts), 300
+    sizes = [int(rng.integers(30, 200)) for _ in range(B)]
+    offsets = _a(np.concatenate([[0], np.cumsum(sizes)]), np.int32)
+    pos_w = _a(rng.normal(0, 3, (int(offsets[-1]), 3)), np.float64)
+    frames, m12s = [], []
+    for b in range(B):
+        n = int(rng.integers(100, cap + 1))
+        frames.append(dict(x=rng.uniform(0, 640, n).astype(np.float32), y=rng.uniform(0, 480, n).astype(np.float32),
+                           octave=rng.integers(0, 8, n).astype(np.int32)))
+        m12s.append(np.where(rng.random(n) < 0.4, rng.integers(0, sizes[b], n), -1).astype(np.int32))
+    n_kp = _a([len(f["x"]) for f in frames], np.int32)
+    X, Y, O = (np.zeros((B, cap), dt) for dt in (np.float32, np.float32, np.int32))
+    matched = np.full((B, cap), -5, np.int32)
+    for b, f in enumerate(frames):
+        n = len(f["x"])
+        X[b, :n], Y[b, :n], O[b, :n], matched[b, :n] = f["x"], f["y"], f["octave"], m12s[b]
+    count = _a(counts, np.int32)
+    pose_in = _a(rng.normal(0, 1, (B, 16)), np.float64)
+    obs = np.zeros((B, cap), oracle_api.PT_OBS_DTYPE)
+    obs_kp, obs_row = np.zeros((B, cap), np.int32), np.zeros((B, cap), np.int32)
+    n_obs, t_in = np.full(B, -3, np.int32), np.full(B, -3, np.int32)
+    isig = _a(ISIG, np.float32)
+    emu.emu_tail_begin(C.c_int(B), C.c_int(cap), _ptr(n_kp), _ptr(X), _ptr(Y), _ptr(O), _ptr(isig), C.c_int(len(isig)),
+                       _ptr(count), None, None, _ptr(pos_w), _ptr(offsets), None, _ptr(pose_in), _ptr(matched),
+                       _ptr(obs), _ptr(obs_kp), _ptr(obs_row), _ptr(n_obs), _ptr(t_in))
+    outlier = (rng.random((B, cap)) < 0.2).astype(np.uint8)
+    num_valid = np.full(B, -3, np.int32)
+    emu.emu_tail_finish(_ptr(outlier), _ptr(num_valid))
+    got = dict(n_obs=n_obs, obs_kp=obs_kp, obs_row=obs_row, obs=obs, matched=matched, num_valid=num_valid,
+               outlier=outlier)
+    assert list(t_in) == list(range(B))
+    for b, f in enumerate(frames):
+        _expect_tail(got, b, counts[b], m12s[b], pos_w[offsets[b]:offsets[b + 1]], f)
+    assert [int(n_obs[b] > 0) for b in range(B)] == [1, 0, 1, 0, 1, 1]
