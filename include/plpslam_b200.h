@@ -798,6 +798,12 @@ PLP_API plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int bat
                                                          uint8_t *d_observable_out, double *d_pose_out,
                                                          int32_t *d_num_tracked_out, int32_t *d_n_inliers_out,
                                                          int32_t *d_lm_iters_out, int32_t *d_status_out);
+/* The window matcher's match count per frame (max_batch entries) in the most recent motion_track_batch_dev (its last
+ * attempt: the widened-margin retry where that ran) and local_map_track_batch_dev (NULL before plp_tracker_reserve_local_map;
+ * a frame the local-map stage skipped keeps an older value): device pointers owned by the tracker, valid once its stream
+ * has reached those calls.  0xffffffff: the frame has more keypoints than the window matcher holds (3072); it matched
+ * nothing, and in the motion track it is not retried and fails. */
+PLP_API plp_status plp_tracker_match_counts(const plp_tracker *t, const uint32_t **d_motion, const uint32_t **d_local);
 
 /* frame_tracker::bow_match_based_track (module/frame_tracker.cc:126-189) against each frame's reference keyframe
  * (curr_frm.ref_keyfrm_), for the frames of the tracker's most recent motion_track_batch_dev that the reference hands to
@@ -858,8 +864,9 @@ PLP_API plp_status plp_tracker_keyframe_bow(const plp_tracker *t, const int32_t 
  * -> essential_solver(frm.bearings_, keyfrm->bearings_, matches).find_via_ransac(50, false) -> the inlier matches;
  * below 20 the frame fails, else pose_optimizer::optimize from last_frm.cam_pose_cw_ -> discard_outliers.  Monocular.
  * Allocates the scratch for max_batch frames; call it once, outside the hot path (a second call replaces the first).
- * Refuses a tracker whose kp_capacity exceeds the brute-force matcher's 4096 (PLP_ERR_INVALID) or the hypothesis
- * kernel's shared memory (PLP_ERR_CAPACITY), before allocating anything. */
+ * Refuses a tracker whose kp_capacity exceeds the hypothesis kernel's shared memory (8 bytes per keypoint;
+ * PLP_ERR_CAPACITY), before allocating anything.  Any kp_capacity is accepted otherwise: the brute-force matcher holds
+ * min(kp_capacity, 4096) keypoints per frame, and a frame with more fails (num_bf_matches_out -1). */
 PLP_API plp_status plp_tracker_reserve_robust_track(plp_tracker *t);
 /* Follows keyframe_track_batch_dev on the same stream (batch <= that call's batch) and reads the keyframe table it was
  * given (rows, desc, valid, pos_w, kf_of_frame, local_idx: keep it alive) and the motion and keyframe calls' outputs and
@@ -871,7 +878,9 @@ PLP_API plp_status plp_tracker_reserve_robust_track(plp_tracker *t);
  *     num_valid >= 20), else 0;
  *   kf_matched_out[batch x kp_capacity]: the keyframe row each keypoint keeps after discard_outliers, or -1;
  *   num_bf_matches_out[batch]: the brute-force match count, num_robust_matches_out[batch]: the RANSAC inliers among
- *     them (0 if the solution is not valid) (both 0 where the stage did not run);
+ *     them (0 if the solution is not valid) (both 0 where the stage did not run); num_bf_matches_out -1: the frame has
+ *     more keypoints than the brute-force matcher holds (4096), matched nothing and fails (pose_last, every other frame
+ *     of the batch unaffected);
  *   pose_out[batch x 16]: the optimiser result, or pose_last where it did not run or found fewer than 20 robust matches;
  *   num_valid_out, n_inliers_out, lm_iters_out [batch] (0 where the optimiser did not run);
  *   status_out[batch]: the keyframe call's status; a frame with status != 0 fails like a track with no match.

@@ -154,4 +154,11 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     return PLP_OK;
 }
 
+plp_status plp_tracker_match_counts(const plp_tracker *t, const uint32_t **d_motion, const uint32_t **d_local) {
+    PLP_REQUIRE(t && d_motion && d_local, "null pointer");
+    *d_motion = t->dev.num_matches;
+    *d_local = t->local ? t->local->num_matches : nullptr;
+    return PLP_OK;
+}
+
 }  // extern "C"

@@ -272,6 +272,12 @@ __global__ void __launch_bounds__(kThreads, 1)
     const BruteJob &J = jobs[blockIdx.x];
     const int tid = threadIdx.x;
     const int n1 = J.n_frm, n2 = J.n_kf;
+    if (n1 > cap) {  // more keypoints than the shared-memory tables hold: report "no matches" loudly (0xffffffff)
+        for (int i = tid; i < n1; i += kThreads) J.matched_out[i] = -1;
+        for (int q = tid; q < n2; q += kThreads) J.choice[q] = -1;
+        if (tid == 0 && J.num_matches) *J.num_matches = 0xffffffffu;
+        return;
+    }
     uint4 *sdesc = reinterpret_cast<uint4 *>(smem_raw);
     int *owner_prev = reinterpret_cast<int *>(smem_raw + (size_t)cap * 32);
     int *owner_next = owner_prev + cap;

@@ -5,6 +5,11 @@
 
 namespace plp {
 
+// Per-frame keypoint capacities of the shared-memory matchers.  A job over its launch's capacity matches nothing and
+// reports the count 0xffffffff.
+constexpr int kMatchMaxPoints = 3072;  // the window matcher (point_match_kernel)
+constexpr int kBruteMaxPoints = 4096;  // the brute-force matcher (brute_match_kernel)
+
 // One CTA per job.  All pointers are device pointers.
 struct PointMatchJob {
     // current frame (candidates)

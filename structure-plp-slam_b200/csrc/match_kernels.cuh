@@ -6,9 +6,6 @@
 
 namespace plp {
 
-constexpr int kMatchMaxPoints = 3072;  // per-frame keypoint capacity of the window matcher (smem bound)
-constexpr int kBruteMaxPoints = 4096;
-
 plp_status launch_point_match(plp_ctx *ctx, const PointMatchJob *d_jobs, int num_jobs, int max_n,
                               const plp_grid &grid, int ratio_test, float lowe_ratio,
                               int check_orientation);

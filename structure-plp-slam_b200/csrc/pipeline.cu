@@ -278,7 +278,7 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
     J.x = T.x;
     J.y = T.y;
     J.octave = T.octave;
-    J.count = (const int32_t *)T.num_matches;  // the matcher's count (uint32_t), far below 2^31
+    J.count = (const int32_t *)T.num_matches;  // the matcher's count (uint32_t); 0xffffffff (over capacity) reads -1
     J.rows = TrackRows{T.last_pos_w, T.last_offsets, nullptr};
     J.pose_in = T.pose_pred;
     J.matched = d_matched_out;

@@ -6,7 +6,8 @@
 // the same stream and without leaving HBM.  It reads the motion and keyframe calls' inputs, outputs and scratch
 // (tracker.h) and writes separate outputs.  Device code: robust_track_kernels.cuh; the brute-force matcher
 // (brute_match_kernel) and the tail (track_common.cuh) are the existing ones, and the eight-point solve and the score
-// are plp_essential_ransac's (essential_common.cuh).
+// are plp_essential_ransac's (essential_common.cuh).  The matcher holds min(cap, kBruteMaxPoints) keypoints per frame;
+// a frame with more fails with num_bf_matches -1 (robust_track_kernels.cuh), so any kp_capacity can be reserved.
 #include "common.cuh"
 #include "match_kernels.cuh"
 #include "robust_track_kernels.cuh"
@@ -28,7 +29,6 @@ extern "C" {
 
 plp_status plp_tracker_reserve_robust_track(plp_tracker *t) {
     PLP_REQUIRE(t, "null pointer");
-    PLP_REQUIRE(t->cap <= kBruteMaxPoints, "kp_capacity exceeds the brute-force matcher's capacity (4096)");
     PLP_CUDA_TRY(cudaSetDevice(t->ctx->device));
     PLP_SMEM_OPTIN(rt::rt_hypothesis_kernel, hypothesis_smem(t->cap));  // one hypothesis' residuals
     if (t->d_rb) {  // a second reservation replaces the first once the stream has stopped using it
@@ -136,7 +136,8 @@ plp_status plp_tracker_robust_track_batch_dev(plp_tracker *t, int batch, const d
 
     PLP_LAUNCH(ctx, rt::rt_prep_kernel, div_up(batch, rt::kPrepThreads), rt::kPrepThreads, 0, D);
     PLP_CHECK_LAUNCH();
-    PLP_TRY(launch_brute_match(ctx, D.bjobs, batch, t->cap, rt::kLoweRatio, 0));
+    PLP_TRY(launch_brute_match(ctx, D.bjobs, batch, t->cap < kBruteMaxPoints ? t->cap : kBruteMaxPoints, rt::kLoweRatio,
+                               0));
     PLP_LAUNCH(ctx, rt::rt_list_kernel, batch, rt::kThreads, 0, D);
     PLP_CHECK_LAUNCH();
     PLP_LAUNCH(ctx, rt::rt_hypothesis_kernel, dim3(rt::kNumIter, batch), rt::kEssThreads, hypothesis_smem(t->cap), D);

@@ -9,7 +9,8 @@
 // Kernels, in launch order (brute_match_kernel in between is the existing one):
 //   rt_prep_kernel        one thread per frame: stage flag, status, the BruteJob (empty for a frame that does not run)
 //   rt_list_kernel        one CTA per frame: the brute-force match list in frame keypoint order, the frame's bearings
-//                         (undistorted tracker), the 50 x 8 sample sets (ransac_sample.h)
+//                         (undistorted tracker), the 50 x 8 sample sets (ransac_sample.h); a frame with more keypoints
+//                         than the matcher holds (kBruteMaxPoints) gets the count -1 and no list, and fails
 //   rt_hypothesis_kernel  grid (50, frames): the eight-point solve and the inlier score of one hypothesis; the residuals
 //                         are staged in shared memory, only E and the score are kept
 //   rt_select_kernel      one CTA per frame: the first-best replay, validity, the winner's inlier flags (recomputed)
@@ -69,7 +70,7 @@ struct RtDev {
     // outputs
     int32_t *stage, *status;           // batch
     int32_t *matched;                  // batch x cap: brute-force matches, then the robust ones (keyframe rows)
-    int32_t *num_bf, *num_robust;      // batch
+    int32_t *num_bf, *num_robust;      // batch; num_bf -1: the frame has more than kBruteMaxPoints keypoints
 };
 
 // the frame runs robust_match_based_track: it needs it and its inputs are in range
@@ -105,14 +106,18 @@ __global__ void __launch_bounds__(kPrepThreads) rt_prep_kernel(RtDev D) {
 
 // robust.cc:371-382: the match list in ascending frame keypoint order; the frame's bearings (frame.cc:79) where the
 // undistortion did not write them; create_random_array(8, 0, M - 1) for each of the 50 hypotheses (-1: none drawn).
+// A frame over the matcher's capacity (robust_track.cu launches it for min(cap, kBruteMaxPoints) keypoints; its guard
+// set every match to -1) lists nothing and reports num_bf = -1, so that the caller can tell it from a frame without a
+// match; with fewer than 8 entries the later kernels leave it as failed.
 __global__ void __launch_bounds__(kThreads) rt_list_kernel(RtDev D) {
     const int b = blockIdx.x, tid = threadIdx.x;
     const size_t base = (size_t)b * D.cap;
     const bool active = frame_active(D, b);
     const int n = active ? D.n_kp[b] : 0;
+    const bool over = n > kBruteMaxPoints;
     const int32_t *matched = D.matched + base;
     int32_t *pairs = D.pairs + 2 * base;
-    const int M = compact_in_order<kThreads>(n, [&](int i) { return matched[i] >= 0; },
+    const int M = compact_in_order<kThreads>(over ? 0 : n, [&](int i) { return matched[i] >= 0; },
                                              [&](int i, int off) {
                                                  pairs[2 * off] = i;
                                                  pairs[2 * off + 1] = matched[i];
@@ -127,7 +132,7 @@ __global__ void __launch_bounds__(kThreads) rt_list_kernel(RtDev D) {
             for (int k = 0; k < 8; ++k) s[k] = -1;
         }
     }
-    if (tid == 0) D.num_bf[b] = M;
+    if (tid == 0) D.num_bf[b] = over ? -1 : M;
 }
 
 // Dynamic shared memory: cap x 2 floats (the residuals of one hypothesis).

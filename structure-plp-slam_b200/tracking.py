@@ -526,6 +526,21 @@ class FrontEnd:
                     status=o["status"].download(np.int32, (batch,)),
                     samples=samples[:batch].copy())
 
+    def download_match_counts(self, batch: int):
+        """The window matcher's per-frame match counts (uint32) of the last track() and track_local_map() (None before
+        reserve_local_map); 0xffffffff: the frame has more keypoints than the matcher holds."""
+        self._after_tracking()
+        m, l = C.c_void_p(), C.c_void_p()
+        self.ctx._check(self.lib.plp_tracker_match_counts(self._trk, C.byref(m), C.byref(l)))
+        out = {}
+        for name, p in (("motion", m), ("local", l)):
+            a = None
+            if p.value:
+                a = np.zeros(batch, np.uint32)
+                self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, a.ctypes.data_as(_P), p, C.c_size_t(a.nbytes)))
+            out[name] = a
+        return out
+
     def download_tracking(self, batch: int):
         self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))

@@ -126,11 +126,13 @@ def oracle_robust_track(orc, cam, curr, kf, frm_bearings, samples, pose_last):
     return out
 
 
-def compare(out, wants, stage, seed, pose_tol=1e-4):
-    """Device results of download_robust_tracking against the oracle's, frame by frame; -> LM iteration lists of the
-    frames that ran the stage."""
+def compare(out, wants, stage, seed, pose_tol=1e-4, frames=None):
+    """Device results of download_robust_tracking against the oracle's, frame by frame (only `frames`, if given); -> LM
+    iteration lists of the frames that ran the stage."""
     got_it, want_it = [], []
     for b, w in enumerate(wants):
+        if frames is not None and b not in frames:
+            continue
         what = f"frame {b}"
         assert out["stage"][b] == stage[b], what
         if not stage[b]:
@@ -150,25 +152,52 @@ def compare(out, wants, stage, seed, pose_tol=1e-4):
     return got_it, want_it
 
 
+def upload_keypoints(fe, res_list):
+    """The frames' keypoints and descriptors written straight into the front end's extraction outputs (in place of
+    extract()), e.g. an extraction with more keypoints than the device extractor's budget allows."""
+    from plpslam_b200.capi import KP_DTYPE
+    B = len(res_list)
+    kp = np.zeros((B, fe.cap), KP_DTYPE)
+    desc = np.zeros((B, fe.cap, 32), np.uint8)
+    n = np.array([len(r["kps"]) for r in res_list], np.int32)
+    assert n.max() <= fe.cap, (n.max(), fe.cap)
+    for b, r in enumerate(res_list):
+        kp[b, :n[b]] = r["kps"]
+        desc[b, :n[b]] = r["desc"]
+    fe.d_kp.upload(kp)
+    fe.d_desc.upload(desc)
+    fe.d_n.upload(n)
+
+
 def run_case(orc, plp, fe, ov, gv, seq, res, ts, kfs, kf_of_frame, motion_valid, fail=(), seed=0, rb_seed=0,
-             grid=None, cam=None, undistort=None):
-    """One batch: motion track (frames in `fail` get a predicted pose a metre off), keyframe track, robust track, then
-    the local-map stage.  Returns dict(mot, kf, kf_wants, kf_stage, rb, rb_wants, rb_stage, local, local_wants)."""
+             grid=None, cam=None, undistort=None, over=(), kps_given=False, fail_shift=(1.0, 0.5, 0.0)):
+    """One batch: motion track (frames in `fail` get a predicted pose shifted by fail_shift), keyframe track, robust
+    track, then the local-map stage.  kps_given: the frames' keypoints are res[t], uploaded (upload_keypoints), and the ORB
+    extractor does not run.  over: frames with more keypoints than the window matcher holds; their motion and local-map
+    results are not compared here (local_wants None) but left to the caller.  Returns dict(mot, kf, kf_wants, kf_stage,
+    rb, rb_wants, rb_stage, local, local_wants, frm_bearings)."""
     rng = np.random.default_rng(seed)
     grid, cam = grid or fe.grid, cam or fe.cam
     preds = [seq.predicted_pose(t, rng) for t in ts]
     for b in fail:
         preds[b] = preds[b].copy()
-        preds[b][:3, 3] += np.array([1.0, 0.5, 0.0])
+        preds[b][:3, 3] += np.asarray(fail_shift)
     lasts = [seq.last_frame_landmarks(t - 1, lmd._kps(res[t - 1], undistort), res[t - 1]["desc"]) for t in ts]
     B = len(ts)
-    fe.upload_images(seq.frames[ts])
     fe.set_last_frames(lasts, np.stack(preds), np.stack([seq.poses[t - 1] for t in ts]))
-    fe.step(B, 20.0)
+    if kps_given:
+        upload_keypoints(fe, [res[t] for t in ts])
+        fe.track(B, 20.0)
+    else:
+        fe.upload_images(seq.frames[ts])
+        fe.step(B, 20.0)
     mot = fe.download_tracking(B)
     curr = [lmd.curr_frame_u(res[t], undistort) for t in ts]
-    motions = [lmd.oracle_motion(orc, grid, cam, curr[b], lasts[b], preds[b], seq.poses[t - 1]) for b, t in enumerate(ts)]
+    motions = [lmd.oracle_motion(orc, grid, cam, curr[b], lasts[b], preds[b], seq.poses[t - 1])
+               if b not in over else None for b, t in enumerate(ts)]
     for b in range(B):
+        if b in over:
+            continue
         assert np.array_equal(motions[b][1], mot["matched"][b]) and motions[b][3] == mot["num_valid"][b], f"motion {b}"
     mv = np.ones(B, np.uint8) if motion_valid is None else np.asarray(motion_valid, np.uint8)
     kf_stage = [int(mv[b] == 0 or mot["num_valid"][b] < NUM_MATCHES_THR) for b in range(B)]
@@ -212,7 +241,9 @@ def run_case(orc, plp, fe, ov, gv, seq, res, ts, kfs, kf_of_frame, motion_valid,
     lout = fe.download_local_tracking(B)
     lwants = []
     for b in range(B):
-        if kf_stage[b]:
+        if b in over:
+            lwants.append(None)
+        elif kf_stage[b]:
             kf = kfs[kf_of_frame[b]]
             loc = dict(local_list[b], last_local_idx=local_idx[b])
             if rb_stage[b]:

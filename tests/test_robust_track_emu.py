@@ -242,3 +242,76 @@ def test_robust_track_kernels_on_cpu_equal_restatement(emu, ess_emu, orc):
     assert num_bf[1] < 8 and valid[1] == 0
     assert valid[2] == 1 and 8 <= num_robust[2] < 20
     assert valid[6] == 1 and num_robust[6] >= 20
+
+
+
+def _run_chain(emu, frames, kfs, kf_of_frame, kf_stage, kf_nv, kf_status, cap, seed):
+    """emu_rt_begin + emu_rt_finish (no outliers) over the frames; -> the outputs as a dict of arrays."""
+    B = len(frames)
+    n_kp = _a([len(f["x"]) for f in frames], np.int32)
+
+    def pad(key, dt, fill=0):
+        out = np.full((B, cap), fill, dt)
+        for b, f in enumerate(frames):
+            out[b, :len(f[key])] = f[key]
+        return out
+    X, Y, O, BF = pad("x", np.float32), pad("y", np.float32), pad("octave", np.int32), pad("bf", np.int32, -9)
+    rows = _a(np.concatenate([[0], np.cumsum([len(k["bearings"]) for k in kfs])]), np.int32)
+    kb = _a(np.concatenate([k["bearings"] for k in kfs]), np.float64)
+    kpos = _a(np.concatenate([k["pos_w"] for k in kfs]), np.float64)
+    pose_last = _a(np.tile(np.eye(4), (B, 1, 1)), np.float64)
+    K = _a([CAM.fx, CAM.fy, CAM.cx, CAM.cy], np.float64)
+    o = dict(bear=np.full((B, cap, 3), -7.0), matched=np.full((B, cap), -5, np.int32),
+             pairs=np.zeros((B, cap, 2), np.int32), samples=np.full((B, 50, 8), -3, np.int32), E=np.zeros((B, 50, 9)),
+             score=np.full((B, 50), -1.0, np.float32), inlier=np.zeros((B, cap), np.uint8), best_score=np.full(B, -1.0),
+             obs=np.zeros((B, cap), oracle_api.PT_OBS_DTYPE), obs_kp=np.zeros((B, cap), np.int32),
+             obs_row=np.zeros((B, cap), np.int32))
+    for k in ("stage", "status", "num_bf", "valid", "num_robust", "n_obs", "num_valid"):
+        o[k] = np.full(B, -3, np.int32)
+    isig = _a(ISIG, np.float32)
+    args = [_a(a, np.int32) for a in (kf_stage, kf_status, kf_nv, kf_of_frame)]
+    emu.emu_rt_begin(C.c_int(B), C.c_int(cap), C.c_uint64(seed), _ptr(n_kp), _ptr(X), _ptr(Y), _ptr(O),
+                     _ptr(pose_last), _ptr(isig), C.c_int(len(isig)), _ptr(K), *[_ptr(a) for a in args], _ptr(rows),
+                     _ptr(kpos), _ptr(kb), _ptr(o["bear"]), C.c_int(1), _ptr(BF), _ptr(o["stage"]), _ptr(o["status"]),
+                     _ptr(o["matched"]), _ptr(o["num_bf"]), _ptr(o["pairs"]), _ptr(o["samples"]), _ptr(o["E"]),
+                     _ptr(o["score"]), _ptr(o["inlier"]), _ptr(o["best_score"]), _ptr(o["valid"]),
+                     _ptr(o["num_robust"]), _ptr(o["obs"]), _ptr(o["obs_kp"]), _ptr(o["obs_row"]), _ptr(o["n_obs"]))
+    emu.emu_rt_finish(_ptr(np.zeros((B, cap), np.uint8)), _ptr(o["num_valid"]))
+    return o
+
+
+def test_robust_frame_over_matcher_capacity(emu):
+    """A frame with more keypoints than the brute-force matcher holds (4096; the matcher's guard leaves every match -1)
+    lists nothing and reports num_bf = -1, draws no sample, gathers nothing and fails.  A frame with exactly 4096
+    keypoints, an over-capacity frame whose keyframe track succeeded (the stage does not run: num_bf 0) and a normal
+    frame are unaffected: they equal the same frames run without the over-capacity frame."""
+    rng = np.random.default_rng(72)
+    f1, k1 = _frame_from_view(rng, 12, 4096)          # 0: exactly the matcher's capacity
+    f2, k0 = _frame_from_view(rng, 13, 4150)          # 1: over it, keyframe stage succeeded
+    f3, _ = _frame_from_view(rng, 14, 120)            # 2: normal
+    f0, _ = _frame_from_view(rng, 11, 4200)           # 3: over it, runs the stage
+    over = dict(f0, bf=np.full(len(f0["bf"]), -1, np.int32))  # what the matcher's guard leaves
+    frames = [f1, f2, f3, over]
+    assert [len(f["x"]) for f in frames] == [4096, 4150, 120, 4200]
+    kfs, kf_of_frame = [k0, k1], [1, 0, 1, 0]
+    kf_stage, kf_nv, kf_status = [1, 1, 1, 1], [0, 25, 3, 0], [0, 0, 0, 0]
+    cap, seed = 4224, 99
+    got = _run_chain(emu, frames, kfs, kf_of_frame, kf_stage, kf_nv, kf_status, cap, seed)
+    ref = _run_chain(emu, frames[:3], kfs, kf_of_frame[:3], kf_stage[:3], kf_nv[:3], kf_status[:3], cap, seed)
+    assert list(got["stage"]) == [1, 0, 1, 1] and list(got["status"]) == [0, 0, 0, 0]
+    # the over-capacity frame: the marker, no list, no samples, no RANSAC, no observations
+    assert got["num_bf"][3] == -1
+    assert (got["samples"][3] == -1).all() and got["valid"][3] == 0 and got["num_robust"][3] == 0
+    assert got["n_obs"][3] == 0 and got["num_valid"][3] == 0 and (got["matched"][3, :4200] == -1).all()
+    # the other frames equal the batch without it
+    for b in range(3):
+        n = len(frames[b]["x"])
+        for k in ("stage", "num_bf", "valid", "num_robust", "n_obs", "num_valid", "best_score"):
+            assert got[k][b] == ref[k][b], (b, k)
+        M = max(int(got["num_bf"][b]), 0)
+        for k in ("samples", "E", "score"):
+            assert np.array_equal(got[k][b], ref[k][b]), (b, k)
+        assert np.array_equal(got["pairs"][b, :M], ref["pairs"][b, :M]), b
+        assert np.array_equal(got["matched"][b, :n], ref["matched"][b, :n]), b
+    assert got["num_bf"][0] == 4096 and got["num_robust"][0] >= 20 and got["num_valid"][0] >= 20
+    assert got["num_bf"][1] == 0 and got["num_bf"][2] == 120
