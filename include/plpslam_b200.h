@@ -788,11 +788,13 @@ PLP_API plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale
  *   status_out: 0, 1 = the frame's local list exceeds max_local_points, 2 = a last_local_idx entry is out of range.
  * After a plp_tracker_keyframe_track_batch_dev of the same batch (batch <= its batch), a frame with stage 1 is taken from
  * that call instead: active iff its keyframe track succeeded, starting from its pose, with the keyframe landmarks its pose
- * optimisation observed excluded through plp_track_keyframe.local_idx, and matched_out holding keyframe rows; status 2
- * if its local_idx block is missing or out of range.
+ * optimisation observed excluded through plp_track_keyframe.local_idx (through the update's blocks when `local` is the
+ * list of plp_tracker_update_local_map_batch_dev), and matched_out holding keyframe rows; status 2 if its local_idx block
+ * is missing or out of range.
  * A frame whose motion track failed, or with status != 0, keeps the motion pose with every per-keypoint output -1, every
  * observable flag 0, 0 iterations and num_tracked 0.  Without a reservation, or with batch > max_batch or no preceding
- * motion track: PLP_ERR_INVALID and nothing is launched. */
+ * motion track, or given the update's list when that update no longer stands or covers fewer frames: PLP_ERR_INVALID
+ * and nothing is launched. */
 PLP_API plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, const plp_track_local *local,
                                                          float margin, int32_t *d_matched_out, int32_t *d_local_out,
                                                          uint8_t *d_observable_out, double *d_pose_out,
@@ -898,6 +900,76 @@ PLP_API plp_status plp_tracker_robust_track_batch_dev(plp_tracker *t, int batch,
  * reached that call.  They are util::create_random_array(8, 0, n - 1) over a counter-based generator keyed by
  * (seed, frame, hypothesis); see csrc/ransac_sample.h. */
 PLP_API plp_status plp_tracker_robust_samples(const plp_tracker *t, const int32_t **d_samples);
+
+/* tracking_module::update_local_map (tracking_module.cc:837-906; module/local_map_updater.cc), monocular points: from
+ * the landmarks each frame has just tracked, its local keyframes, its local landmark list (the plp_track_local that
+ * local_map_track_batch_dev takes) and its nearest covisibility (the new reference keyframe).  The map is a snapshot the
+ * caller owns and keeps alive; keyframes and landmarks are indexed by table position.  Keyframe indices double as the
+ * canonical order of the first-level keyframes, which the reference visits in pointer-hash order: fill the table in
+ * keyframe::id_ order (see DESIGN.md). */
+typedef struct plp_track_map { /* device pointers; L landmarks, K keyframes                                           */
+    /* landmarks */
+    const double *pos_w, *obs_mean_normal;                             /* L x 3                                     */
+    const float *min_valid_dist, *max_valid_dist, *max_valid_dist_raw; /* L: get_min/max_valid_distance(), max_valid_dist_ */
+    const uint8_t *desc;                                               /* L x 32, 4-byte aligned                    */
+    const uint8_t *lm_erased;                                          /* L: will_be_erased()                       */
+    const int32_t *obs_offsets;                                        /* L + 1: landmark l's get_observations() are */
+    const int32_t *obs_kf;                                             /*   obs_kf[obs_offsets[l] .. obs_offsets[l+1]) (distinct) */
+    /* keyframes */
+    const uint8_t *kf_erased;                                          /* K: will_be_erased()                       */
+    const int32_t *row_offsets;                                        /* K + 1: keyframe k's get_landmarks() are    */
+    const int32_t *row_lm;                                             /*   row_lm[row_offsets[k] ..] (-1: none)     */
+    const int32_t *cov_offsets, *cov_kf;                               /* K + 1, get_top_n_covisibilities(10) in order */
+    const int32_t *child_offsets, *child_kf;                           /* K + 1, get_spanning_children() in order   */
+    const int32_t *parent;                                             /* K: get_spanning_parent(), -1 = none       */
+    /* the rows of the tracking stages */
+    const int32_t *last_row_lm;    /* per plp_track_last row (motion call): its landmark, or -1                     */
+    const int32_t *kf_row_lm;      /* per plp_track_keyframe row (keyframe call): its landmark, or -1; NULL without one */
+} plp_track_map;
+
+/* Allocates the update's outputs and scratch for max_batch frames: the local list (max_batch x max_local_points rows
+ * of every plp_track_local field, max_local_points from plp_tracker_reserve_local_map, which must come first), the
+ * last_local_idx rows (max_batch x max_last_points) and, when plp_tracker_reserve_keyframe_track came first, the
+ * keyframe local_idx blocks (max_batch x max_keyframe_points), and the per-frame vote and dedup tables.
+ * max_local_keyframes >= 64 bounds the distinct keyframes a frame's tracked landmarks may vote for.  A vote table the
+ * device's shared memory cannot hold: PLP_ERR_CAPACITY, nothing allocated.  Call it once, outside the hot path (a
+ * second call replaces the first). */
+PLP_API plp_status plp_tracker_reserve_local_map_update(plp_tracker *t, int max_local_keyframes);
+/* Follows the last tracking call of the batch (motion, keyframe or robust) on the same stream, batch <= that call's
+ * batch, and precedes local_map_track_batch_dev; no host synchronisation.  For every frame the local-map stage would
+ * start (the same start record; num_valid >= 20 and its status 0): the tracked keypoints whose landmark is not erased
+ * vote for the landmark's observers; the non-erased voted keyframes in ascending index are the first level (uncapped),
+ * nearest = the largest vote (ties: lowest index); the second level adds, for each first-level keyframe while the list
+ * holds at most 60, the first new non-erased covisibility, spanning child and the parent; the local landmarks are the
+ * local keyframes' non-null, non-erased rows in order, first occurrence kept.  Outputs (device, caller-owned):
+ *   nearest_out[batch]: keyframe index, or -1;
+ *   local_kf_out[batch x max_local_keyframes], num_local_kf_out[batch]: the local keyframes;
+ *   local_lm_out[max_batch x max_local_points]: the landmark of every row of the local list;
+ *   status_out[batch]: 0, 1 = the local list exceeds max_local_points, 2 = more voted keyframes than
+ *     max_local_keyframes, 3 = no keyframe voted (the reference keeps its previous local map, which the device does
+ *     not hold).  A frame with status != 0, or that the local-map stage skips, has an empty local list, nearest -1 and
+ *     every mapping -1; the caller handles status != 0 on the host.
+ * The list itself is tracker-owned: plp_tracker_updated_local_map.  It comes with keyframe local_idx blocks: a
+ * local_map_track_batch_dev given that list maps the keyframe and robust stages' rows through them, in place of
+ * plp_track_keyframe.local_idx; one given another list uses plp_track_keyframe.local_idx as before.  A later motion,
+ * keyframe or robust call, or a new reservation, ends the list: a local-map call given it then fails with
+ * PLP_ERR_INVALID.  The tracking records are never changed.  Without a reservation, without a preceding
+ * motion call, with batch above the last tracking call's, with kf_row_lm NULL after a keyframe call, with a null
+ * required array, a map desc that is not 4-byte aligned, or after a later plp_tracker_reserve_local_map, or a plp_tracker_reserve_keyframe_track with more
+ * points, than the update's reservation was made for: PLP_ERR_INVALID and nothing is launched. */
+PLP_API plp_status plp_tracker_update_local_map_batch_dev(plp_tracker *t, int batch, const plp_track_map *map,
+                                                          int32_t *d_nearest_out, int32_t *d_local_kf_out,
+                                                          int32_t *d_num_local_kf_out, int32_t *d_local_lm_out,
+                                                          int32_t *d_status_out);
+/* The plp_track_local of the most recent update_local_map_batch_dev (offsets: batch + 1, contiguous; last_local_idx: one
+ * entry per plp_track_last row): device pointers owned by the tracker, valid once its stream has reached that call.
+ * PLP_ERR_INVALID when no update stands. */
+PLP_API plp_status plp_tracker_updated_local_map(const plp_tracker *t, plp_track_local *out);
+/* The keyframe local_idx blocks of the same update (what a local-map call given its list reads): per frame that
+ * starts from one of those stages with status 0, one entry per row of its keyframe-table keyframe, else none;
+ * local_idx_offsets has batch + 1 entries.  Tracker-owned, like the list. */
+PLP_API plp_status plp_tracker_updated_local_idx(const plp_tracker *t, const int32_t **d_local_idx,
+                                                 const int32_t **d_local_idx_offsets);
 
 /* ------------------------------------------------------------------------ */
 /* local bundle adjustment (optimize/local_bundle_adjuster*.cc)               */

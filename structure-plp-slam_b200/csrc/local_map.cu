@@ -103,6 +103,11 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     PLP_REQUIRE(!t->record_batch[kStageRobust] || t->covers(kStageRobust, batch),
                 "the batch must not exceed that of the plp_tracker_robust_track_batch_dev that followed the keyframe track");
     PLP_REQUIRE(margin > 0.0f, "margin");
+    // the list of plp_tracker_update_local_map_batch_dev (local_map_update.cu) comes with its own keyframe local_idx
+    // blocks; it is taken only while that update stands and over at most its batch
+    const bool from_update = t->d_upd && local->offsets == t->updated.offsets;
+    PLP_REQUIRE(!from_update || (t->update_batch && batch <= t->update_batch),
+                "the list of plp_tracker_update_local_map_batch_dev no longer stands or covers fewer frames");
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     const TrackDev &M = t->motion;
@@ -119,6 +124,10 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.motion.local_idx_offsets = M.last_offsets;
     if (t->record_batch[kStageKeyframe]) D.kf = t->record[kStageKeyframe];  // else D.kf.stage stays null
     if (t->record_batch[kStageRobust]) D.rb = t->record[kStageRobust];      // else D.rb.stage stays null
+    if (from_update) {  // keyframe rows map into the update's list through its blocks, not plp_track_keyframe.local_idx
+        D.kf.local_idx = D.rb.local_idx = t->upd_local_idx;
+        D.kf.local_idx_offsets = D.rb.local_idx_offsets = t->upd_local_idx_offsets;
+    }
     D.pos_w = local->pos_w;
     D.normal = local->obs_mean_normal;
     D.min_d = local->min_valid_dist;

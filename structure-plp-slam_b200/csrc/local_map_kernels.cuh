@@ -86,12 +86,8 @@ struct LocalDev {
     int32_t *num_tracked, *n_inliers, *lm_iters, *status;  // batch
 };
 
-// The record the frame starts from: the robust track where it ran, else the keyframe track where it ran, else the
-// motion track.  The robust track runs only where the keyframe track ran.
-__device__ __forceinline__ bool ran(const TrackRecord &R, int b) { return R.stage && R.stage[b]; }
-__device__ __forceinline__ const TrackRecord &start(const LocalDev &D, int b) {
-    return ran(D.rb, b) ? D.rb : ran(D.kf, b) ? D.kf : D.motion;
-}
+// the record the frame starts from (track_common.cuh; the local-map update chooses it the same way)
+__device__ __forceinline__ const TrackRecord &start(const LocalDev &D, int b) { return start_record(D, b); }
 
 // the frame runs the stage: its tracker succeeded and its inputs are in range
 __device__ __forceinline__ bool frame_active(const LocalDev &D, int b) {

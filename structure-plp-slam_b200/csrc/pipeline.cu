@@ -218,6 +218,7 @@ void plp_tracker_destroy(plp_tracker *t) {
     if (t->d_local) cudaFree(t->d_local);
     if (t->d_kf) cudaFree(t->d_kf);
     if (t->d_rb) cudaFree(t->d_rb);
+    if (t->d_upd) cudaFree(t->d_upd);
     delete t;
 }
 

@@ -17,6 +17,15 @@ constexpr int kTailThreads = 256;   // gather / finish: one CTA per frame
 // frame b's block of rows
 __device__ __forceinline__ int row_block(const TrackRows &R, int b) { return R.of_frame ? R.of_frame[b] : b; }
 
+// The record a frame starts its local-map work from, for a job holding the batch's records as motion, kf and rb: the
+// robust track where it ran, else the keyframe track where it ran, else the motion track.  The robust track runs only
+// where the keyframe track ran.  A keyframe or robust record that does not stand has stage == nullptr.
+__device__ __forceinline__ bool ran(const TrackRecord &R, int b) { return R.stage && R.stage[b]; }
+template <class Job>
+__device__ __forceinline__ const TrackRecord &start_record(const Job &D, int b) {
+    return ran(D.rb, b) ? D.rb : ran(D.kf, b) ? D.kf : D.motion;
+}
+
 struct TrackTail {
     int cap;
     // the current frames' keypoints (undistorted, SoA: batch x cap)

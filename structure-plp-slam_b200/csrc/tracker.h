@@ -1,6 +1,7 @@
 // tracker.h -- internal: the state of a plp_tracker, shared by its stages, which run in order on a batch:
 // pipeline.cu (motion_based_track), keyframe_track.cu (bow_match_based_track), robust_track.cu
-// (robust_match_based_track) and local_map.cu (optimize_current_frame_with_local_map).  Each of the first three ends in
+// (robust_match_based_track), local_map_update.cu (update_local_map) and local_map.cu
+// (optimize_current_frame_with_local_map).  Each of the first three ends in
 // the same tail (track_common.cuh) and leaves a TrackRecord (track_record.h) that the later stages of the batch read.
 #pragma once
 #include <memory>
@@ -21,6 +22,9 @@ struct KfDev;  // keyframe_track_kernels.cuh
 }
 namespace rt {
 struct RtDev;  // robust_track_kernels.cuh
+}
+namespace lu {
+struct UpdDev;  // local_map_update_kernels.cuh
 }
 
 struct TrackDev {
@@ -81,9 +85,11 @@ struct plp_tracker {
     plp::TrackTail tail[plp::kNumStages];
     plp::TrackRecord record[plp::kNumStages];
     int record_batch[plp::kNumStages] = {};
-    // a call of stage s, or a new reservation for it, ends the records of s and of every later stage
+    // a call of stage s, or a new reservation for it, ends the records of s and of every later stage, and the local-map
+    // update built on them
     void invalidate_from(int s) {
         for (; s < plp::kNumStages; ++s) record_batch[s] = 0;
+        update_batch = 0;
     }
     // stage s left a record that covers the first `batch` (>= 1) frames
     bool covers(int s, int batch) const { return batch <= record_batch[s]; }
@@ -108,4 +114,14 @@ struct plp_tracker {
     // robust tracking (plp_tracker_reserve_robust_track); d_rb == nullptr until reserved
     uint8_t *d_rb = nullptr;         // one allocation, carved by robust_track.cu
     std::shared_ptr<plp::rt::RtDev> rb;
+    // local-map update (plp_tracker_reserve_local_map_update); d_upd == nullptr until reserved
+    uint8_t *d_upd = nullptr;        // one allocation, carved by local_map_update.cu
+    std::shared_ptr<plp::lu::UpdDev> upd;
+    int upd_max_kf_points = 0;       // the keyframe rows its local_idx blocks hold
+    // the update's list (pointers fixed by the reservation) and its keyframe local_idx blocks, which a local-map call
+    // given that list reads in place of plp_track_keyframe.local_idx; the records themselves are never changed
+    plp_track_local updated{};
+    const int32_t *upd_local_idx = nullptr, *upd_local_idx_offsets = nullptr;
+    // the batch of the most recent update, 0 once none stands (a tracking call or a new reservation ends it)
+    int update_batch = 0;
 };
