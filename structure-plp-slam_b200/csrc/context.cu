@@ -73,6 +73,7 @@ plp_status stage(plp_ctx *ctx, int slot, DevLayout &L) {
 cudaError_t alloc(plp_ctx *ctx, DevLayout &L, uint8_t **block, bool zero) {
     cudaError_t e = cudaMalloc((void **)block, L.bytes());
     if (e != cudaSuccess) {
+        cudaGetLastError();  // the caller reports the refusal; a later launch check must not report it again
         *block = nullptr;
         return e;
     }

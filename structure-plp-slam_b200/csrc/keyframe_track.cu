@@ -45,6 +45,8 @@ size_t job_smem(int cap) { return (size_t)cap * (sizeof(unsigned long long) + si
 
 }  // namespace
 
+int32_t *keyframe_choice(const plp_tracker *t) { return t->kf->choice; }
+
 }  // namespace plp
 
 using namespace plp;
@@ -56,10 +58,7 @@ plp_status plp_tracker_reserve_keyframe_track(plp_tracker *t, int max_keyframes,
     PLP_REQUIRE(max_keyframes >= 1 && max_keyframe_points >= 1, "max_keyframes / max_keyframe_points");
     PLP_CUDA_TRY(cudaSetDevice(t->ctx->device));
     PLP_SMEM_OPTIN(kt::kf_job_kernel, job_smem(t->cap));  // the feature-vector kernel's cap x 12 bytes
-    if (t->d_kf) {  // a second reservation replaces the first once the stream has stopped using it
-        PLP_CUDA_TRY(cudaStreamSynchronize(t->ctx->stream));
-        cudaFree(t->d_kf);
-        t->d_kf = nullptr;
+    if (t->kf) {  // a second reservation ends the first, and what was tracked with it
         t->max_keyframes = t->max_kf_points = 0;
         t->invalidate_from(kStageKeyframe);
     }
@@ -81,21 +80,12 @@ plp_status plp_tracker_reserve_keyframe_track(plp_tracker *t, int max_keyframes,
     L.out(D->m21, B * R);
     L.out(D->bjobs, B);
     TrackTail J = t->tail[kStageMotion];  // the tracker's cap and inv_level_sigma_sq; this stage's scratch
-    L.out(J.posejobs, B);
-    L.out(J.obs, B * C);
-    L.out(J.obs_kp, B * C);
-    L.out(J.obs_row, B * C);
-    L.out(J.obs_outlier, B * C);
-    if (alloc(t->ctx, L, &t->d_kf, false) != cudaSuccess) {
-        set_error("tracker: cudaMalloc(%zu) for keyframe tracking failed", L.bytes());
-        return PLP_ERR_CUDA;
-    }
-    t->max_keyframes = max_keyframes;
-    t->max_kf_points = max_keyframe_points;
+    tail_scratch(L, J, B, C);
     D->cap = t->cap;
     D->max_kf_points = max_keyframe_points;
-    t->kf = D;
-    t->kf_choice = D->choice;
+    PLP_TRY(t->kf.reserve(t->ctx, L, D, "keyframe tracking"));
+    t->max_keyframes = max_keyframes;
+    t->max_kf_points = max_keyframe_points;
     t->tail[kStageKeyframe] = J;
     return PLP_OK;
 }
@@ -113,18 +103,16 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
                     kf->node_ids && kf->node_begin && kf->indices,
                 "keyframe arrays");
     PLP_REQUIRE(!kf->local_idx == !kf->local_idx_offsets, "local_idx and local_idx_offsets go together");
-    PLP_REQUIRE(t->d_kf, "plp_tracker_reserve_keyframe_track has not been called");
+    PLP_REQUIRE(t->kf, "plp_tracker_reserve_keyframe_track has not been called");
     PLP_REQUIRE(kf->num_keyframes >= 0 && kf->num_keyframes <= t->max_keyframes,
                 "num_keyframes exceeds the reserved max_keyframes");
-    PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
-    PLP_REQUIRE(t->covers(kStageMotion, batch),
-                "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
+    PLP_TRY(t->check_order(kStageKeyframe, batch));
     PLP_REQUIRE(vocab->ctx->device == t->ctx->device, "the vocabulary lives on another device");
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     t->invalidate_from(kStageKeyframe);
     const TrackDev &M = t->motion;
-    KfDev D = *t->kf;
+    KfDev D = *t->kf.job;
     D.batch = batch;
     D.num_keyframes = kf->num_keyframes;
     D.n_kp = M.n_kp;
@@ -146,21 +134,13 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
     D.matched = d_kf_matched_out;
     D.num_bow = (uint32_t *)d_num_bow_matches_out;
     // pose-opt from last_frm.cam_pose_cw_ over the frames with 20 BoW matches (frame_tracker.cc:138-169)
-    TrackTail J = t->tail[kStageKeyframe];
-    J.n_kp = M.n_kp;
-    J.x = M.x;
-    J.y = M.y;
-    J.octave = M.octave;
+    TrackTail J = t->tail_job(kStageKeyframe, d_kf_matched_out, d_pose_out, d_num_valid_out, d_n_inliers_out,
+                              d_lm_iters_out);
     J.count = d_num_bow_matches_out;
     J.stage = d_stage_out;
     J.status = d_status_out;
     J.rows = TrackRows{kf->pos_w, kf->row_offsets, kf->kf_of_frame};
     J.pose_in = M.pose_last;
-    J.matched = d_kf_matched_out;
-    J.pose = d_pose_out;
-    J.num_valid = d_num_valid_out;
-    J.n_inliers = d_n_inliers_out;
-    J.lm_iters = d_lm_iters_out;
 
     PLP_LAUNCH(ctx, kt::kf_prep_kernel, div_up(batch, kt::kPrepThreads), kt::kPrepThreads, 0, D);
     PLP_CHECK_LAUNCH();
@@ -178,7 +158,7 @@ plp_status plp_tracker_keyframe_track_batch_dev(plp_tracker *t, plp_bow_vocab *v
 plp_status plp_tracker_keyframe_bow(const plp_tracker *t, const int32_t **d_word_id, const int32_t **d_node_id,
                                     const float **d_weight) {
     PLP_REQUIRE(t && d_word_id && d_node_id && d_weight, "null pointer");
-    PLP_REQUIRE(t->d_kf, "plp_tracker_reserve_keyframe_track has not been called");
+    PLP_REQUIRE(t->kf, "plp_tracker_reserve_keyframe_track has not been called");
     *d_word_id = t->kf->word;
     *d_node_id = t->kf->node;
     *d_weight = t->kf->weight;

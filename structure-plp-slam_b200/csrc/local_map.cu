@@ -39,12 +39,7 @@ plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale_factor,
     float thr[16];
     PLP_TRY(plp_fuse_level_thresholds(log_scale_factor, t->num_levels, thr));
     PLP_CUDA_TRY(cudaSetDevice(t->ctx->device));
-    if (t->d_local) {  // a second reservation replaces the first once the stream has stopped using it
-        PLP_CUDA_TRY(cudaStreamSynchronize(t->ctx->stream));
-        cudaFree(t->d_local);
-        t->d_local = nullptr;
-        t->max_local = 0;
-    }
+    t->max_local = 0;
     // the scratch of every later call, bound once (B frames, C keypoints, ML local rows)
     const size_t B = t->max_batch, C = t->cap, ML = max_local_points;
     auto D = std::make_shared<LocalDev>();
@@ -67,20 +62,16 @@ plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale_factor,
     L.out(D->obs, B * C);
     L.out(D->obs_kp, B * C);
     L.out(D->obs_outlier, B * C);
-    if (alloc(t->ctx, L, &t->d_local, false) != cudaSuccess) {
-        set_error("tracker: cudaMalloc(%zu) for the local map failed", L.bytes());
-        return PLP_ERR_CUDA;
-    }
-    t->max_local = max_local_points;
     D->cap = t->cap;
-    D->max_local = t->max_local;
+    D->max_local = max_local_points;
     D->cam = t->cam;
     for (int l = 0; l < 16; ++l) {
         D->scale_factors[l] = l < t->num_levels ? t->scale_factors[l] : 1.0f;
         D->level_thr[l] = l < t->num_levels ? thr[l] : INFINITY;
     }
     D->num_levels = t->num_levels;
-    t->local = D;
+    PLP_TRY(t->local.reserve(t->ctx, L, D, "the local map"));
+    t->max_local = max_local_points;
     return PLP_OK;
 }
 
@@ -94,24 +85,18 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     PLP_REQUIRE(local->pos_w && local->obs_mean_normal && local->min_valid_dist && local->max_valid_dist &&
                     local->max_valid_dist_raw && local->desc && local->offsets && local->last_local_idx,
                 "local-map arrays");
-    PLP_REQUIRE(t->d_local, "plp_tracker_reserve_local_map has not been called");
-    PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
-    PLP_REQUIRE(t->covers(kStageMotion, batch),
-                "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
-    PLP_REQUIRE(!t->record_batch[kStageKeyframe] || t->covers(kStageKeyframe, batch),
-                "the batch must not exceed that of the plp_tracker_keyframe_track_batch_dev that followed the motion track");
-    PLP_REQUIRE(!t->record_batch[kStageRobust] || t->covers(kStageRobust, batch),
-                "the batch must not exceed that of the plp_tracker_robust_track_batch_dev that followed the keyframe track");
+    PLP_REQUIRE(t->local, "plp_tracker_reserve_local_map has not been called");
+    PLP_TRY(t->check_order(kNumStages, batch));
     PLP_REQUIRE(margin > 0.0f, "margin");
     // the list of plp_tracker_update_local_map_batch_dev (local_map_update.cu) comes with its own keyframe local_idx
     // blocks; it is taken only while that update stands and over at most its batch
-    const bool from_update = t->d_upd && local->offsets == t->updated.offsets;
+    const bool from_update = t->upd && local->offsets == t->updated.offsets;
     PLP_REQUIRE(!from_update || (t->update_batch && batch <= t->update_batch),
                 "the list of plp_tracker_update_local_map_batch_dev no longer stands or covers fewer frames");
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     const TrackDev &M = t->motion;
-    LocalDev D = *t->local;
+    LocalDev D = *t->local.job;
     D.batch = batch;
     D.n_kp = M.n_kp;
     D.x = M.x;
@@ -122,8 +107,8 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.motion = t->record[kStageMotion];
     D.motion.local_idx = local->last_local_idx;  // one entry per last-frame row
     D.motion.local_idx_offsets = M.last_offsets;
-    if (t->record_batch[kStageKeyframe]) D.kf = t->record[kStageKeyframe];  // else D.kf.stage stays null
-    if (t->record_batch[kStageRobust]) D.rb = t->record[kStageRobust];      // else D.rb.stage stays null
+    D.kf = t->standing(kStageKeyframe);
+    D.rb = t->standing(kStageRobust);
     if (from_update) {  // keyframe rows map into the update's list through its blocks, not plp_track_keyframe.local_idx
         D.kf.local_idx = D.rb.local_idx = t->upd_local_idx;
         D.kf.local_idx_offsets = D.rb.local_idx_offsets = t->upd_local_idx_offsets;

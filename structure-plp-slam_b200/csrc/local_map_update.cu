@@ -31,20 +31,16 @@ extern "C" {
 
 plp_status plp_tracker_reserve_local_map_update(plp_tracker *t, int max_local_keyframes) {
     PLP_REQUIRE(t, "null pointer");
-    PLP_REQUIRE(t->d_local, "plp_tracker_reserve_local_map has not been called");
+    PLP_REQUIRE(t->local, "plp_tracker_reserve_local_map has not been called");
     PLP_REQUIRE(max_local_keyframes >= lu::kMinReservedKeyframes && max_local_keyframes <= (1 << 20),
                 "max_local_keyframes must be at least 64");
     PLP_CUDA_TRY(cudaSetDevice(t->ctx->device));
     const int vote_slots = pow2_at_least(2LL * max_local_keyframes);
     PLP_SMEM_OPTIN(lu::lmu_vote_kernel, lu::vote_smem_bytes(vote_slots, max_local_keyframes));
-    if (t->d_upd) {  // a second reservation replaces the first once the stream has stopped using it
-        PLP_CUDA_TRY(cudaStreamSynchronize(t->ctx->stream));
-        cudaFree(t->d_upd);
-        t->d_upd = nullptr;
-        t->update_batch = 0;
-        t->updated = plp_track_local{};
-        t->upd_local_idx = t->upd_local_idx_offsets = nullptr;
-    }
+    // a second reservation ends the first's list
+    t->update_batch = 0;
+    t->updated = plp_track_local{};
+    t->upd_local_idx = t->upd_local_idx_offsets = nullptr;
     // the scratch and tracker-owned outputs of every later call, bound once (B frames, ML local rows, LK local
     // keyframes, S landmark slots, M last rows, R keyframe rows)
     const size_t B = t->max_batch, ML = t->max_local, LK = max_local_keyframes, M = t->max_last, R = t->max_kf_points;
@@ -72,16 +68,12 @@ plp_status plp_tracker_reserve_local_map_update(plp_tracker *t, int max_local_ke
     L.out(D->last_local_idx, B * M);
     L.out(D->local_idx, R ? B * R : 1);
     L.out(D->local_idx_offsets, B + 1);
-    if (alloc(t->ctx, L, &t->d_upd, false) != cudaSuccess) {
-        set_error("tracker: cudaMalloc(%zu) for the local-map update failed", L.bytes());
-        return PLP_ERR_CUDA;
-    }
     D->cap = t->cap;
     D->max_local = t->max_local;
     D->max_lkf = max_local_keyframes;
     D->vote_slots = vote_slots;
     D->lm_slots = lm_slots;
-    t->upd = D;
+    PLP_TRY(t->upd.reserve(t->ctx, L, D, "the local-map update"));
     t->upd_max_kf_points = t->max_kf_points;
     plp_track_local &out = t->updated;  // the list every later call writes
     out.pos_w = D->pos_w;
@@ -110,33 +102,27 @@ plp_status plp_tracker_update_local_map_batch_dev(plp_tracker *t, int batch, con
                     map->child_offsets && map->child_kf && map->parent && map->last_row_lm,
                 "map arrays");
     PLP_REQUIRE(((uintptr_t)map->desc & 3) == 0, "map desc must be 4-byte aligned");
-    PLP_REQUIRE(t->d_upd, "plp_tracker_reserve_local_map_update has not been called");
+    PLP_REQUIRE(t->upd, "plp_tracker_reserve_local_map_update has not been called");
     PLP_REQUIRE(t->upd->max_local == t->max_local,
                 "plp_tracker_reserve_local_map was called again after plp_tracker_reserve_local_map_update");
-    PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
-    PLP_REQUIRE(t->covers(kStageMotion, batch),
-                "the batch must follow a plp_tracker_motion_track_batch_dev of at least as many frames");
-    const bool kf = t->record_batch[kStageKeyframe] != 0, rb = t->record_batch[kStageRobust] != 0;
-    PLP_REQUIRE(!kf || t->covers(kStageKeyframe, batch),
-                "the batch must not exceed that of the plp_tracker_keyframe_track_batch_dev that followed the motion track");
-    PLP_REQUIRE(!rb || t->covers(kStageRobust, batch),
-                "the batch must not exceed that of the plp_tracker_robust_track_batch_dev that followed the keyframe track");
+    PLP_TRY(t->check_order(kNumStages, batch));
+    const bool kf = t->record_batch[kStageKeyframe] != 0;
     PLP_REQUIRE(!kf || map->kf_row_lm, "kf_row_lm is required after a plp_tracker_keyframe_track_batch_dev");
     PLP_REQUIRE(!kf || t->max_kf_points <= t->upd_max_kf_points,
                 "plp_tracker_reserve_keyframe_track was called with more points after plp_tracker_reserve_local_map_update");
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
-    UpdDev D = *t->upd;
+    UpdDev D = *t->upd.job;
     D.batch = batch;
     D.n_kp = t->motion.n_kp;
     D.last_offsets = t->motion.last_offsets;
     D.motion = t->record[kStageMotion];
+    D.kf = t->standing(kStageKeyframe);
+    D.rb = t->standing(kStageRobust);
     if (kf) {
-        D.kf = t->record[kStageKeyframe];  // else D.kf.stage stays null
         D.kf_of_frame = t->kf_table.kf_of_frame;
         D.kf_row_offsets = t->kf_table.row_offsets;
     }
-    if (rb) D.rb = t->record[kStageRobust];  // else D.rb.stage stays null
     D.map = *map;
     D.nearest = d_nearest_out;
     D.local_kf = d_local_kf_out;

@@ -176,11 +176,7 @@ plp_status plp_tracker_create_ex(plp_ctx *ctx, const plp_camera *cam, const plp_
     memset(&J, 0, sizeof(J));
     J.cap = kp_capacity;
     for (int l = 0; l < 16; ++l) J.inv_level_sigma_sq[l] = l < num_levels ? inv_level_sigma_sq[l] : 1.0f;
-    L.out(J.posejobs, B);
-    L.out(J.obs, B * C);
-    L.out(J.obs_kp, B * C);
-    L.out(J.obs_outlier, B * C);
-    L.out(J.obs_row, B * C);
+    tail_scratch(L, J, B, C);
     if (distorted) {
         t->distorted = true;
         t->undist = uj;
@@ -213,12 +209,12 @@ plp_status plp_tracker_undistorted(const plp_tracker *t, const plp_keypoint **d_
 void plp_tracker_destroy(plp_tracker *t) {
     if (!t) return;
     cudaSetDevice(t->ctx->device);
+    t->local.release(t->ctx->stream);
+    t->kf.release(t->ctx->stream);
+    t->rb.release(t->ctx->stream);
+    t->upd.release(t->ctx->stream);
     cudaStreamSynchronize(t->ctx->stream);
     if (t->d_block) cudaFree(t->d_block);
-    if (t->d_local) cudaFree(t->d_local);
-    if (t->d_kf) cudaFree(t->d_kf);
-    if (t->d_rb) cudaFree(t->d_rb);
-    if (t->d_upd) cudaFree(t->d_upd);
     delete t;
 }
 
@@ -229,7 +225,7 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
     PLP_REQUIRE(t && d_kp && d_desc && d_n_kp && last && d_matched_out && d_pose_out && d_num_valid_out &&
                     d_n_inliers_out && d_lm_iters_out,
                 "null pointer");
-    PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
+    PLP_TRY(t->check_order(kStageMotion, batch));
     PLP_REQUIRE(last->pos_w && last->octave && last->angle && last->desc && last->offsets && last->pose_pred &&
                     last->pose_last,
                 "last-frame arrays");
@@ -274,21 +270,12 @@ plp_status plp_tracker_motion_track_batch_dev(plp_tracker *t, int batch, const p
     PLP_TRY(launch_point_match(ctx, T.mjobs + batch, batch, t->cap > kMatchMaxPoints ? kMatchMaxPoints : t->cap, t->grid,
                                0, 0.0f, 1));
     // pose-opt from the predicted pose over the frames with 20 matches (frame_tracker.cc:73-108)
-    TrackTail J = t->tail[kStageMotion];
-    J.n_kp = d_n_kp;
-    J.x = T.x;
-    J.y = T.y;
-    J.octave = T.octave;
+    t->motion = T;
+    TrackTail J = t->tail_job(kStageMotion, d_matched_out, d_pose_out, d_num_valid_out, d_n_inliers_out, d_lm_iters_out);
     J.count = (const int32_t *)T.num_matches;  // the matcher's count (uint32_t); 0xffffffff (over capacity) reads -1
     J.rows = TrackRows{T.last_pos_w, T.last_offsets, nullptr};
     J.pose_in = T.pose_pred;
-    J.matched = d_matched_out;
-    J.pose = d_pose_out;
-    J.num_valid = d_num_valid_out;
-    J.n_inliers = d_n_inliers_out;
-    J.lm_iters = d_lm_iters_out;
     PLP_TRY(launch_track_tail(ctx, J, batch, t->cam));
-    t->motion = T;
     t->set_record(kStageMotion, batch, J, nullptr, nullptr);  // local_map.cu binds last_local_idx
     return PLP_OK;
 }

@@ -31,12 +31,7 @@ plp_status plp_tracker_reserve_robust_track(plp_tracker *t) {
     PLP_REQUIRE(t, "null pointer");
     PLP_CUDA_TRY(cudaSetDevice(t->ctx->device));
     PLP_SMEM_OPTIN(rt::rt_hypothesis_kernel, hypothesis_smem(t->cap));  // one hypothesis' residuals
-    if (t->d_rb) {  // a second reservation replaces the first once the stream has stopped using it
-        PLP_CUDA_TRY(cudaStreamSynchronize(t->ctx->stream));
-        cudaFree(t->d_rb);
-        t->d_rb = nullptr;
-        t->invalidate_from(kStageRobust);
-    }
+    if (t->rb) t->invalidate_from(kStageRobust);  // a second reservation ends what was tracked with the first
     // the scratch of every later call, bound once (B frames, C keypoints, K hypotheses)
     const size_t B = t->max_batch, C = t->cap, K = rt::kNumIter;
     auto D = std::make_shared<rt::RtDev>();
@@ -52,15 +47,7 @@ plp_status plp_tracker_reserve_robust_track(plp_tracker *t) {
     L.out(D->valid, B);
     if (!t->distorted) L.out(D->bearings, B * C * 3);  // a distorted tracker's undistortion writes them
     TrackTail J = t->tail[kStageMotion];  // the tracker's cap and inv_level_sigma_sq; this stage's scratch
-    L.out(J.posejobs, B);
-    L.out(J.obs, B * C);
-    L.out(J.obs_kp, B * C);
-    L.out(J.obs_row, B * C);
-    L.out(J.obs_outlier, B * C);
-    if (alloc(t->ctx, L, &t->d_rb, false) != cudaSuccess) {
-        set_error("tracker: cudaMalloc(%zu) for robust tracking failed", L.bytes());
-        return PLP_ERR_CUDA;
-    }
+    tail_scratch(L, J, B, C);
     D->cap = t->cap;
     if (t->distorted) {
         D->bearings = t->d_bearings;
@@ -71,7 +58,7 @@ plp_status plp_tracker_reserve_robust_track(plp_tracker *t) {
         D->K_cfg[2] = t->cam.cx;
         D->K_cfg[3] = t->cam.cy;
     }
-    t->rb = D;
+    PLP_TRY(t->rb.reserve(t->ctx, L, D, "robust tracking"));
     t->tail[kStageRobust] = J;
     return PLP_OK;
 }
@@ -85,17 +72,15 @@ plp_status plp_tracker_robust_track_batch_dev(plp_tracker *t, int batch, const d
                     d_num_robust_matches_out && d_pose_out && d_num_valid_out && d_n_inliers_out && d_lm_iters_out &&
                     d_status_out,
                 "null pointer");
-    PLP_REQUIRE(t->d_rb, "plp_tracker_reserve_robust_track has not been called");
-    PLP_REQUIRE(batch >= 1 && batch <= t->max_batch, "batch exceeds the tracker's max_batch");
-    PLP_REQUIRE(t->covers(kStageKeyframe, batch),
-                "the batch must follow a plp_tracker_keyframe_track_batch_dev of at least as many frames");
+    PLP_REQUIRE(t->rb, "plp_tracker_reserve_robust_track has not been called");
+    PLP_TRY(t->check_order(kStageRobust, batch));
     plp_ctx *ctx = t->ctx;
     PLP_CUDA_TRY(cudaSetDevice(ctx->device));
     t->invalidate_from(kStageRobust);
     const TrackDev &M = t->motion;
     const TrackRecord &KT = t->record[kStageKeyframe];
     const plp_track_keyframe &tab = t->kf_table;
-    rt::RtDev D = *t->rb;
+    rt::RtDev D = *t->rb.job;
     D.batch = batch;
     D.seed = seed;
     D.max_kf_points = t->max_kf_points;
@@ -111,28 +96,20 @@ plp_status plp_tracker_robust_track_batch_dev(plp_tracker *t, int batch, const d
     D.kf_desc = tab.desc;
     D.kf_valid = tab.valid;
     D.kf_bearings = d_kf_bearings;
-    D.choice = t->kf_choice;  // the keyframe call's matcher scratch (max_batch x max_keyframe_points), free again now
+    D.choice = keyframe_choice(t);
     D.stage = d_stage_out;
     D.status = d_status_out;
     D.matched = d_kf_matched_out;
     D.num_bf = d_num_bf_matches_out;
     D.num_robust = d_num_robust_matches_out;
     // pose-opt from last_frm.cam_pose_cw_ over the frames with 20 robust matches (frame_tracker.cc:203-245)
-    TrackTail J = t->tail[kStageRobust];
-    J.n_kp = M.n_kp;
-    J.x = M.x;
-    J.y = M.y;
-    J.octave = M.octave;
+    TrackTail J = t->tail_job(kStageRobust, d_kf_matched_out, d_pose_out, d_num_valid_out, d_n_inliers_out,
+                              d_lm_iters_out);
     J.count = d_num_robust_matches_out;
     J.stage = d_stage_out;
     J.status = d_status_out;
     J.rows = KT.rows;  // the keyframe call's rows and kf_of_frame
     J.pose_in = M.pose_last;
-    J.matched = d_kf_matched_out;
-    J.pose = d_pose_out;
-    J.num_valid = d_num_valid_out;
-    J.n_inliers = d_n_inliers_out;
-    J.lm_iters = d_lm_iters_out;
 
     PLP_LAUNCH(ctx, rt::rt_prep_kernel, div_up(batch, rt::kPrepThreads), rt::kPrepThreads, 0, D);
     PLP_CHECK_LAUNCH();
@@ -151,7 +128,7 @@ plp_status plp_tracker_robust_track_batch_dev(plp_tracker *t, int batch, const d
 
 plp_status plp_tracker_robust_samples(const plp_tracker *t, const int32_t **d_samples) {
     PLP_REQUIRE(t && d_samples, "null pointer");
-    PLP_REQUIRE(t->d_rb, "plp_tracker_reserve_robust_track has not been called");
+    PLP_REQUIRE(t->rb, "plp_tracker_reserve_robust_track has not been called");
     *d_samples = t->rb->samples;
     return PLP_OK;
 }

@@ -48,6 +48,33 @@ def _logf(x: float) -> float:
     return float(libm.logf(float(np.float32(x))))
 
 
+class _Packed:
+    """Per-item arrays end to end, as the C ABI takes a ragged list (one item per frame or keyframe): item i's rows are
+    [offsets[i], offsets[i + 1]), and `count` is the key whose length gives an item's rows."""
+
+    def __init__(self, items, count: str):
+        self.items = items
+        self.offsets = np.zeros(len(items) + 1, np.int32)
+        self.offsets[1:] = np.cumsum([len(it[count]) for it in items])
+
+    def cat(self, key: str, dtype, shape=(), fill=None) -> np.ndarray:
+        """The items' `key` arrays (rows of `shape`) end to end; with `fill`, an item whose `key` is missing or None
+        contributes its rows of that value."""
+        parts = [np.full(n, fill, dtype) if fill is not None and it.get(key) is None else
+                 np.asarray(it[key], dtype).reshape((-1,) + shape) for it, n in zip(self.items, np.diff(self.offsets))]
+        return np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0,) + shape, dtype))
+
+
+def _by_frame(n, a: np.ndarray) -> list:
+    """Frame b's first n[b] rows of a (frames x ...) array, for every frame b < len(n)."""
+    return [a[b, :n[b]].copy() for b in range(len(n))]
+
+
+def _unpack(offsets, a: np.ndarray) -> list:
+    """Item i's rows [offsets[i], offsets[i + 1]) of a packed array, for every i < len(offsets) - 1."""
+    return [a[offsets[i]:offsets[i + 1]].copy() for i in range(len(offsets) - 1)]
+
+
 class DeviceBuffer:
     """A cudaMalloc'ed block owned through the C ABI (plp_dev_alloc / plp_dev_free)."""
 
@@ -142,28 +169,16 @@ class FrontEnd:
         h = C.c_void_p()
         sf = np.ascontiguousarray(self.orb.scale_factors, np.float32)
         isig = np.ascontiguousarray(self.orb.inv_level_sigma_sq, np.float32)
-        if distortion is None:
-            ctx._check(self.lib.plp_tracker_create(self.track_ctx.handle, C.byref(cam), C.byref(self.grid),
-                                                   sf.ctypes.data_as(_P), isig.ctypes.data_as(_P), C.c_int(num_levels),
-                                                   C.c_int(max_batch), C.c_int(self.cap), C.c_int(max_last_points),
-                                                   C.byref(h)))
-        else:
-            ctx._check(self.lib.plp_tracker_create_ex(self.track_ctx.handle, C.byref(cam), C.byref(self.grid),
-                                                      sf.ctypes.data_as(_P), isig.ctypes.data_as(_P), C.c_int(num_levels),
-                                                      C.c_int(max_batch), C.c_int(self.cap), C.c_int(max_last_points),
-                                                      C.byref(distortion), C.byref(h)))
+        ctx._check(self.lib.plp_tracker_create_ex(self.track_ctx.handle, C.byref(cam), C.byref(self.grid),
+                                                  sf.ctypes.data_as(_P), isig.ctypes.data_as(_P), C.c_int(num_levels),
+                                                  C.c_int(max_batch), C.c_int(self.cap), C.c_int(max_last_points),
+                                                  None if distortion is None else C.byref(distortion), C.byref(h)))
         self._trk = h
-        B = max_batch
-        self.d_imgs = DeviceBuffer(ctx, B * rows * cols)
-        self.d_kp = DeviceBuffer(ctx, B * self.cap * KP_DTYPE.itemsize)
-        self.d_desc = DeviceBuffer(ctx, B * self.cap * 32)
-        self.d_n = DeviceBuffer(ctx, B * 4)
-        self.d_status = DeviceBuffer(ctx, B * 4)
-        self.d_matched = DeviceBuffer(ctx, B * self.cap * 4)
-        self.d_pose = DeviceBuffer(ctx, B * 128)
-        self.d_num_valid = DeviceBuffer(ctx, B * 4)
-        self.d_n_inl = DeviceBuffer(ctx, B * 4)
-        self.d_lm = DeviceBuffer(ctx, B * 4)
+        self._motion_out = self._frame_buffers(imgs=rows * cols, kp=self.cap * KP_DTYPE.itemsize, desc=self.cap * 32,
+                                               n_kp=4, status=4, matched=self.cap * 4, pose=128, num_valid=4,
+                                               n_inliers=4, lm_iters=4)
+        (self.d_imgs, self.d_kp, self.d_desc, self.d_n, self.d_status, self.d_matched, self.d_pose, self.d_num_valid,
+         self.d_n_inl, self.d_lm) = self._motion_out.values()
         self.scale_factor = scale_factor
         self._local_bufs = []
         self._local = None
@@ -184,13 +199,18 @@ class FrontEnd:
         self._pin_out = None
         self._out_layout = None
 
+    def _frame_buffers(self, **frame_bytes) -> dict:
+        """One device buffer of max_batch x `frame_bytes[name]` bytes per name; close() frees them."""
+        return {name: DeviceBuffer(self.ctx, self.max_batch * n) for name, n in frame_bytes.items()}
+
     def close(self):
-        for b in self._local_bufs + self._kf_bufs + self._map_bufs:
-            b.free()
-        self._local_bufs = []
-        self._kf_bufs = []
-        self._map_bufs = []
-        self._kf_bearings = None
+        """Frees the tracker and every device and pinned buffer this FrontEnd still holds; a buffer a caller has taken
+        out of its hands (by replacing the attribute) is the caller's.  A second call does nothing."""
+        outs = [o for o in (self._motion_out, self._local_out, self._kf_out, self._rb_out, self._upd_out) if o]
+        for b in ([b for o in outs for b in o.values()] + self._last_bufs + self._last_pinned + self._local_bufs +
+                  self._kf_bufs + self._map_bufs + [self._pin_imgs, self._pin_out]):
+            if b is not None:
+                b.free()
         if self._trk is not None:
             self.lib.plp_tracker_destroy(self._trk)
             self._trk = None
@@ -204,15 +224,12 @@ class FrontEnd:
         """last_list[b]: dict(pos_w[m,3], octave[m], angle[m], desc[m,32], valid[m]|None)."""
         for b in self._last_bufs:
             b.free()
-        offs = np.zeros(len(last_list) + 1, np.int32)
-        offs[1:] = np.cumsum([len(l["octave"]) for l in last_list])
+        last = _Packed(last_list, "octave")
+        offs = last.offsets
         assert max(np.diff(offs)) <= self.max_last
-        cat = lambda k, dt: np.ascontiguousarray(np.concatenate([np.asarray(l[k], dt) for l in last_list]))
-        arrays = [cat("pos_w", np.float64), cat("octave", np.int32), cat("angle", np.float32), cat("desc", np.uint8),
-                  np.ascontiguousarray(np.concatenate([np.asarray(l.get("valid") if l.get("valid") is not None else
-                                                                  np.ones(len(l["octave"]), np.uint8), np.uint8)
-                                                       for l in last_list])),
-                  offs, np.ascontiguousarray(pose_pred, np.float64), np.ascontiguousarray(pose_last, np.float64)]
+        arrays = [last.cat("pos_w", np.float64, (3,)), last.cat("octave", np.int32), last.cat("angle", np.float32),
+                  last.cat("desc", np.uint8, (32,)), last.cat("valid", np.uint8, fill=1), offs,
+                  np.ascontiguousarray(pose_pred, np.float64), np.ascontiguousarray(pose_last, np.float64)]
         self._last_bufs = [DeviceBuffer.from_array(self.ctx, a) for a in arrays]
         self._last = TrackLast(*[b.ptr for b in self._last_bufs])
         self._last_offsets = offs
@@ -226,12 +243,9 @@ class FrontEnd:
         self.ctx._check(self.lib.plp_tracker_reserve_local_map(self._trk, C.c_float(_logf(self.scale_factor)),
                                                            C.c_int(max_local_points)))
         self.max_local = int(max_local_points)
-        B = self.max_batch
         if self._local_out is None:
-            self._local_out = dict(matched=DeviceBuffer(self.ctx, B * self.cap * 4),
-                                   local=DeviceBuffer(self.ctx, B * self.cap * 4), pose=DeviceBuffer(self.ctx, B * 128),
-                                   num_tracked=DeviceBuffer(self.ctx, B * 4), n_inliers=DeviceBuffer(self.ctx, B * 4),
-                                   lm_iters=DeviceBuffer(self.ctx, B * 4), status=DeviceBuffer(self.ctx, B * 4))
+            self._local_out = self._frame_buffers(matched=self.cap * 4, local=self.cap * 4, pose=128, num_tracked=4,
+                                                  n_inliers=4, lm_iters=4, status=4)
 
     def set_local_maps(self, local_list):
         """local_list[b]: dict(pos_w[m,3], normal[m,3] (get_obs_mean_normal), min_valid_dist[m], max_valid_dist[m]
@@ -240,18 +254,12 @@ class FrontEnd:
         local_landmarks_ order."""
         for b in self._local_bufs:
             b.free()
-        offs = np.zeros(len(local_list) + 1, np.int32)
-        offs[1:] = np.cumsum([len(l["max_valid_dist"]) for l in local_list])
-
-        def cat(k, dt, shape):
-            parts = [np.asarray(l[k], dt).reshape((-1,) + shape) for l in local_list]
-            return np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0,) + shape, dt))
-        valid = np.ascontiguousarray(np.concatenate(
-            [np.asarray(l["valid"], np.uint8) if l.get("valid") is not None else np.ones(len(l["max_valid_dist"]), np.uint8)
-             for l in local_list]))
-        arrays = [cat("pos_w", np.float64, (3,)), cat("normal", np.float64, (3,)), cat("min_valid_dist", np.float32, ()),
-                  cat("max_valid_dist", np.float32, ()), cat("max_valid_dist_raw", np.float32, ()),
-                  cat("desc", np.uint8, (32,)), valid, offs, cat("last_local_idx", np.int32, ())]
+        loc = _Packed(local_list, "max_valid_dist")
+        offs = loc.offsets
+        arrays = [loc.cat("pos_w", np.float64, (3,)), loc.cat("normal", np.float64, (3,)),
+                  loc.cat("min_valid_dist", np.float32), loc.cat("max_valid_dist", np.float32),
+                  loc.cat("max_valid_dist_raw", np.float32), loc.cat("desc", np.uint8, (32,)),
+                  loc.cat("valid", np.uint8, fill=1), offs, loc.cat("last_local_idx", np.int32)]
         self._local_bufs = [DeviceBuffer.from_array(self.ctx, a) for a in arrays]
         self._local = TrackLocal(*[b.ptr for b in self._local_bufs])
         self._local_offsets = offs
@@ -263,13 +271,9 @@ class FrontEnd:
         hot path), and the outputs of track_keyframe."""
         self.ctx._check(self.lib.plp_tracker_reserve_keyframe_track(self._trk, C.c_int(max_keyframes),
                                                                     C.c_int(max_keyframe_points)))
-        B = self.max_batch
         if self._kf_out is None:
-            self._kf_out = dict(stage=DeviceBuffer(self.ctx, B * 4), matched=DeviceBuffer(self.ctx, B * self.cap * 4),
-                                num_bow=DeviceBuffer(self.ctx, B * 4), pose=DeviceBuffer(self.ctx, B * 128),
-                                num_valid=DeviceBuffer(self.ctx, B * 4), n_inliers=DeviceBuffer(self.ctx, B * 4),
-                                lm_iters=DeviceBuffer(self.ctx, B * 4), status=DeviceBuffer(self.ctx, B * 4),
-                                motion_valid=DeviceBuffer(self.ctx, B))
+            self._kf_out = self._frame_buffers(stage=4, matched=self.cap * 4, num_bow=4, pose=128, num_valid=4,
+                                               n_inliers=4, lm_iters=4, status=4, motion_valid=1)
 
     def set_keyframes(self, keyframes, kf_of_frame, local_idx=None):
         """keyframes[k]: dict(desc[n,32], angle[n] (keypts_[i].angle), valid[n]|None (lm && !will_be_erased()),
@@ -279,60 +283,43 @@ class FrontEnd:
         per frame, one entry per row of its keyframe -- that landmark's index in the frame's local list, or -1."""
         for b in self._kf_bufs:
             b.free()
-        rows = np.zeros(len(keyframes) + 1, np.int32)
-        rows[1:] = np.cumsum([len(k["desc"]) for k in keyframes])
-        fv_offs = np.zeros(len(keyframes) + 1, np.int32)
-        fv_offs[1:] = np.cumsum([len(k["fv"][0]) for k in keyframes])
+        kfs = _Packed(keyframes, "desc")
+        fv = _Packed([dict(zip(("node_ids", "node_offsets", "indices"), k["fv"])) for k in keyframes], "node_ids")
         node_begin, base = [], 0
-        for k in keyframes:
-            node_begin.append(np.asarray(k["fv"][1][:-1], np.int64) + base)
-            base += len(k["fv"][2])
+        for f in fv.items:
+            node_begin.append(np.asarray(f["node_offsets"][:-1], np.int64) + base)
+            base += len(f["indices"])
         node_begin = np.concatenate(node_begin + [np.array([base])]).astype(np.int32)
-
-        def cat(key, dt, shape):
-            parts = [np.asarray(k[key], dt).reshape((-1,) + shape) for k in keyframes]
-            return np.ascontiguousarray(np.concatenate(parts) if parts else np.zeros((0,) + shape, dt))
-        valid = np.ascontiguousarray(np.concatenate(
-            [np.asarray(k["valid"], np.uint8) if k.get("valid") is not None else np.ones(len(k["desc"]), np.uint8)
-             for k in keyframes]))
-        fv = lambda i, dt: np.ascontiguousarray(np.concatenate([np.asarray(k["fv"][i], dt) for k in keyframes]))
-        arrays = [np.ascontiguousarray(kf_of_frame, np.int32), rows, cat("desc", np.uint8, (32,)),
-                  cat("angle", np.float32, ()), valid, cat("pos_w", np.float64, (3,)), fv_offs, fv(0, np.uint32),
-                  node_begin, fv(2, np.uint32)]
+        arrays = [np.ascontiguousarray(kf_of_frame, np.int32), kfs.offsets, kfs.cat("desc", np.uint8, (32,)),
+                  kfs.cat("angle", np.float32), kfs.cat("valid", np.uint8, fill=1), kfs.cat("pos_w", np.float64, (3,)),
+                  fv.offsets, fv.cat("node_ids", np.uint32), node_begin, fv.cat("indices", np.uint32)]
         if local_idx is not None:
-            lio = np.zeros(len(local_idx) + 1, np.int32)
-            lio[1:] = np.cumsum([len(x) for x in local_idx])
-            arrays += [np.ascontiguousarray(np.concatenate([np.asarray(x, np.int32) for x in local_idx])), lio]
+            li = _Packed([dict(local_idx=x) for x in local_idx], "local_idx")
+            arrays += [li.cat("local_idx", np.int32), li.offsets]
         self._kf_bufs = [DeviceBuffer.from_array(self.ctx, a) for a in arrays]
         ptrs = [b.ptr for b in self._kf_bufs] + [None] * (12 - len(self._kf_bufs))
         self._kf = TrackKeyframe(len(keyframes), *ptrs)
         self._kf_bearings = None
         if keyframes and all(k.get("bearings") is not None for k in keyframes):
-            self._kf_bearings = DeviceBuffer.from_array(self.ctx, cat("bearings", np.float64, (3,)))
+            self._kf_bearings = DeviceBuffer.from_array(self.ctx, kfs.cat("bearings", np.float64, (3,)))
             self._kf_bufs.append(self._kf_bearings)
 
     def reserve_robust_track(self):
         """Scratch of track_robust (outside the hot path), and its outputs."""
         self.ctx._check(self.lib.plp_tracker_reserve_robust_track(self._trk))
-        B = self.max_batch
         if self._rb_out is None:
-            self._rb_out = dict(stage=DeviceBuffer(self.ctx, B * 4), matched=DeviceBuffer(self.ctx, B * self.cap * 4),
-                                num_bf=DeviceBuffer(self.ctx, B * 4), num_robust=DeviceBuffer(self.ctx, B * 4),
-                                pose=DeviceBuffer(self.ctx, B * 128), num_valid=DeviceBuffer(self.ctx, B * 4),
-                                n_inliers=DeviceBuffer(self.ctx, B * 4), lm_iters=DeviceBuffer(self.ctx, B * 4),
-                                status=DeviceBuffer(self.ctx, B * 4))
+            self._rb_out = self._frame_buffers(stage=4, matched=self.cap * 4, num_bf=4, num_robust=4, pose=128,
+                                               num_valid=4, n_inliers=4, lm_iters=4, status=4)
 
     def reserve_local_map_update(self, max_local_keyframes: int = 128):
         """Scratch and list of update_local_map (outside the hot path; after reserve_local_map and, where the keyframe
         stage runs, reserve_keyframe_track), and its per-frame outputs."""
         self.ctx._check(self.lib.plp_tracker_reserve_local_map_update(self._trk, C.c_int(max_local_keyframes)))
         self.max_local_keyframes = int(max_local_keyframes)
-        B, ML = self.max_batch, self.max_local
         for b in (self._upd_out or {}).values():
             b.free()
-        self._upd_out = dict(nearest=DeviceBuffer(self.ctx, B * 4), local_kf=DeviceBuffer(self.ctx, B * max_local_keyframes * 4),
-                             num_local_kf=DeviceBuffer(self.ctx, B * 4), local_lm=DeviceBuffer(self.ctx, B * ML * 4),
-                             status=DeviceBuffer(self.ctx, B * 4), observable=DeviceBuffer(self.ctx, B * ML))
+        self._upd_out = self._frame_buffers(nearest=4, local_kf=max_local_keyframes * 4, num_local_kf=4,
+                                            local_lm=self.max_local * 4, status=4, observable=self.max_local)
 
     def set_map(self, snapshot):
         """The map snapshot update_local_map reads (plp_track_map), keyframes and landmarks by table index:
@@ -443,9 +430,7 @@ class FrontEnd:
         update_local_map() built on the device instead of the one set_local_maps() uploaded."""
         o = self._local_out
         if updated:
-            local = TrackLocal()
-            self.ctx._check(self.lib.plp_tracker_updated_local_map(self._trk, C.byref(local)))
-            observable = self._upd_out["observable"]
+            local, observable = self._updated_list(), self._upd_out["observable"]
         else:
             if o is None or self._local is None:
                 raise PlpError("track_local_map needs reserve_local_map() and set_local_maps() first")
@@ -503,12 +488,29 @@ class FrontEnd:
         if self.track_ctx is not self.ctx:
             self.ctx.wait(self.track_ctx)
 
+    def _tail_results(self, batch: int, o: dict, valid: str = "num_valid") -> dict:
+        """What every tracking call returns per frame, from its outputs `o`: pose, the valid count, n_inliers, LM
+        iterations and status."""
+        return dict(pose=o["pose"].download(np.float64, (batch, 4, 4)),
+                    **{k: o[k].download(np.int32, (batch,)) for k in (valid, "n_inliers", "lm_iters", "status")})
+
+    def _keypoint_rows(self, n, buf: DeviceBuffer, dtype=np.int32) -> list:
+        """Per frame b < len(n), the values of its n[b] keypoints in a max_batch x cap buffer."""
+        return _by_frame(n, buf.download(dtype, (self.max_batch, self.cap)))
+
+    def _download_ptr(self, p, dtype, shape) -> np.ndarray:
+        """An array of `shape` read from the device address p (an int or a c_void_p)."""
+        a = np.zeros(shape, dtype)
+        if a.nbytes:
+            self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, a.ctypes.data_as(_P), C.c_void_p(p),
+                                                      C.c_size_t(a.nbytes)))
+        return a
+
     def download_keypoints(self, batch: int):
         self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
-        kp = self.d_kp.download(KP_DTYPE, (self.max_batch, self.cap))[:batch]
-        desc = self.d_desc.download(np.uint8, (self.max_batch, self.cap, 32))[:batch]
-        return [(kp[b, :n[b]].copy(), desc[b, :n[b]].copy()) for b in range(batch)]
+        return list(zip(self._keypoint_rows(n, self.d_kp, KP_DTYPE),
+                        _by_frame(n, self.d_desc.download(np.uint8, (self.max_batch, self.cap, 32)))))
 
     def download_undistorted(self, batch: int):
         """Per frame (undistorted keypoints, bearings) of the last track() -- frame::undist_keypts_ and bearings_.
@@ -517,14 +519,10 @@ class FrontEnd:
             raise PlpError("FrontEnd without distortion: the ORB keypoints are the undistorted keypoints")
         kp_p, b_p = C.c_void_p(), C.c_void_p()
         self.ctx._check(self.lib.plp_tracker_undistorted(self._trk, C.byref(kp_p), C.byref(b_p)))
+        self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
-        if self.track_ctx is not self.ctx:
-            self.ctx.wait(self.track_ctx)
-        kp = np.zeros((batch, self.cap), KP_DTYPE)
-        bear = np.zeros((batch, self.cap, 3), np.float64)
-        self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, kp.ctypes.data_as(_P), kp_p, C.c_size_t(kp.nbytes)))
-        self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, bear.ctypes.data_as(_P), b_p, C.c_size_t(bear.nbytes)))
-        return [(kp[b, :n[b]].copy(), bear[b, :n[b]].copy()) for b in range(batch)]
+        return list(zip(_by_frame(n, self._download_ptr(kp_p.value, KP_DTYPE, (batch, self.cap))),
+                        _by_frame(n, self._download_ptr(b_p.value, np.float64, (batch, self.cap, 3)))))
 
     def download_local_tracking(self, batch: int):
         """Results of track_local_map: per frame the last-frame row / local-list index held by each keypoint, the
@@ -532,34 +530,20 @@ class FrontEnd:
         self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
         o = self._local_out
-        matched = o["matched"].download(np.int32, (self.max_batch, self.cap))[:batch]
-        local = o["local"].download(np.int32, (self.max_batch, self.cap))[:batch]
         if self._local_from_update:
             offs = self._download_updated_offsets(batch)
             obs = self._upd_out["observable"].download(np.uint8, (max(int(offs[-1]), 1),))
         else:
             offs = self._local_offsets
             obs = self._d_observable.download(np.uint8, (max(int(offs[-1]), 1),))
-        return dict(matched=[matched[b, :n[b]].copy() for b in range(batch)],
-                    local=[local[b, :n[b]].copy() for b in range(batch)],
-                    observable=[obs[offs[b]:offs[b + 1]].copy() for b in range(batch)],
-                    pose=o["pose"].download(np.float64, (batch, 4, 4)),
-                    num_tracked=o["num_tracked"].download(np.int32, (batch,)),
-                    n_inliers=o["n_inliers"].download(np.int32, (batch,)),
-                    lm_iters=o["lm_iters"].download(np.int32, (batch,)),
-                    status=o["status"].download(np.int32, (batch,)))
+        return dict(matched=self._keypoint_rows(n, o["matched"]), local=self._keypoint_rows(n, o["local"]),
+                    observable=_unpack(offs[:batch + 1], obs),
+                    **self._tail_results(batch, o, valid="num_tracked"))
 
     def _updated_list(self) -> TrackLocal:
         local = TrackLocal()
         self.ctx._check(self.lib.plp_tracker_updated_local_map(self._trk, C.byref(local)))
         return local
-
-    def _download_ptr(self, p, dtype, shape) -> np.ndarray:
-        a = np.zeros(shape, dtype)
-        if a.nbytes:
-            self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, a.ctypes.data_as(_P), C.c_void_p(p),
-                                                      C.c_size_t(a.nbytes)))
-        return a
 
     def _download_updated_offsets(self, batch: int) -> np.ndarray:
         return self._download_ptr(self._updated_list().offsets, np.int32, (batch + 1,))
@@ -573,7 +557,7 @@ class FrontEnd:
         loc = self._updated_list()
         offs = self._download_ptr(loc.offsets, np.int32, (batch + 1,))
         n = int(offs[-1])
-        lk = o["local_kf"].download(np.int32, (self.max_batch, self.max_local_keyframes))[:batch]
+        lk = o["local_kf"].download(np.int32, (self.max_batch, self.max_local_keyframes))
         nlk = o["num_local_kf"].download(np.int32, (batch,))
         lm = o["local_lm"].download(np.int32, (max(n, 1),))[:n]
         rows = dict(pos_w=self._download_ptr(loc.pos_w, np.float64, (n, 3)),
@@ -583,19 +567,17 @@ class FrontEnd:
                     max_valid_dist_raw=self._download_ptr(loc.max_valid_dist_raw, np.float32, (n,)),
                     desc=self._download_ptr(loc.desc, np.uint8, (n, 32)),
                     valid=self._download_ptr(loc.valid, np.uint8, (n,)))
-        lo = self._last_offsets
+        lo = self._last_offsets[:batch + 1]
         lli = self._download_ptr(loc.last_local_idx, np.int32, (int(lo[batch]),))
-        out = dict(status=o["status"].download(np.int32, (batch,)), nearest=o["nearest"].download(np.int32, (batch,)),
-                   local_kf=[lk[b, :nlk[b]].copy() for b in range(batch)], offsets=offs,
-                   local_lm=[lm[offs[b]:offs[b + 1]].copy() for b in range(batch)],
-                   rows=[{k: v[offs[b]:offs[b + 1]].copy() for k, v in rows.items()} for b in range(batch)],
-                   last_local_idx=[lli[lo[b]:lo[b + 1]].copy() for b in range(batch)], local_idx=None)
         li, lio = C.c_void_p(), C.c_void_p()
         self.ctx._check(self.lib.plp_tracker_updated_local_idx(self._trk, C.byref(li), C.byref(lio)))
         lio = self._download_ptr(lio.value, np.int32, (batch + 1,))
         li = self._download_ptr(li.value, np.int32, (int(lio[-1]),))
-        out["local_idx"] = [li[lio[b]:lio[b + 1]].copy() for b in range(batch)]
-        return out
+        rows = {k: _unpack(offs, v) for k, v in rows.items()}
+        return dict(status=o["status"].download(np.int32, (batch,)), nearest=o["nearest"].download(np.int32, (batch,)),
+                    local_kf=_by_frame(nlk, lk), offsets=offs, local_lm=_unpack(offs, lm),
+                    rows=[{k: v[b] for k, v in rows.items()} for b in range(batch)],
+                    last_local_idx=_unpack(lo, lli), local_idx=_unpack(lio, li))
 
     def download_keyframe_tracking(self, batch: int):
         """Results of track_keyframe: per frame the stage flag, the keyframe row kept on each keypoint, the BoW match
@@ -604,23 +586,13 @@ class FrontEnd:
         self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
         o = self._kf_out
-        matched = o["matched"].download(np.int32, (self.max_batch, self.cap))[:batch]
         w, nd, wt = C.c_void_p(), C.c_void_p(), C.c_void_p()
         self.ctx._check(self.lib.plp_tracker_keyframe_bow(self._trk, C.byref(w), C.byref(nd), C.byref(wt)))
-        bow = []
-        for p, dt in ((w, np.int32), (nd, np.int32), (wt, np.float32)):
-            a = np.zeros((self.max_batch, self.cap), dt)
-            self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, a.ctypes.data_as(_P), p, C.c_size_t(a.nbytes)))
-            bow.append(a)
-        return dict(stage=o["stage"].download(np.int32, (batch,)),
-                    matched=[matched[b, :n[b]].copy() for b in range(batch)],
-                    num_bow_matches=o["num_bow"].download(np.int32, (batch,)),
-                    pose=o["pose"].download(np.float64, (batch, 4, 4)),
-                    num_valid=o["num_valid"].download(np.int32, (batch,)),
-                    n_inliers=o["n_inliers"].download(np.int32, (batch,)),
-                    lm_iters=o["lm_iters"].download(np.int32, (batch,)),
-                    status=o["status"].download(np.int32, (batch,)),
-                    bow=[tuple(a[b, :n[b]].copy() for a in bow) for b in range(batch)])
+        bow = [_by_frame(n, self._download_ptr(p.value, dt, (batch, self.cap)))
+               for p, dt in ((w, np.int32), (nd, np.int32), (wt, np.float32))]
+        return dict(stage=o["stage"].download(np.int32, (batch,)), matched=self._keypoint_rows(n, o["matched"]),
+                    num_bow_matches=o["num_bow"].download(np.int32, (batch,)), **self._tail_results(batch, o),
+                    bow=list(zip(*bow)))
 
     def download_robust_tracking(self, batch: int):
         """Results of track_robust: per frame the stage flag, the keyframe row kept on each keypoint, the brute-force
@@ -629,22 +601,12 @@ class FrontEnd:
         self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
         o = self._rb_out
-        matched = o["matched"].download(np.int32, (self.max_batch, self.cap))[:batch]
         p = C.c_void_p()
         self.ctx._check(self.lib.plp_tracker_robust_samples(self._trk, C.byref(p)))
-        samples = np.zeros((self.max_batch, 50, 8), np.int32)
-        self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, samples.ctypes.data_as(_P), p,
-                                                  C.c_size_t(samples.nbytes)))
-        return dict(stage=o["stage"].download(np.int32, (batch,)),
-                    matched=[matched[b, :n[b]].copy() for b in range(batch)],
+        return dict(stage=o["stage"].download(np.int32, (batch,)), matched=self._keypoint_rows(n, o["matched"]),
                     num_bf_matches=o["num_bf"].download(np.int32, (batch,)),
-                    num_robust_matches=o["num_robust"].download(np.int32, (batch,)),
-                    pose=o["pose"].download(np.float64, (batch, 4, 4)),
-                    num_valid=o["num_valid"].download(np.int32, (batch,)),
-                    n_inliers=o["n_inliers"].download(np.int32, (batch,)),
-                    lm_iters=o["lm_iters"].download(np.int32, (batch,)),
-                    status=o["status"].download(np.int32, (batch,)),
-                    samples=samples[:batch].copy())
+                    num_robust_matches=o["num_robust"].download(np.int32, (batch,)), **self._tail_results(batch, o),
+                    samples=self._download_ptr(p.value, np.int32, (batch, 50, 8)))
 
     def download_match_counts(self, batch: int):
         """The window matcher's per-frame match counts (uint32) of the last track() and track_local_map() (None before
@@ -652,22 +614,10 @@ class FrontEnd:
         self._after_tracking()
         m, l = C.c_void_p(), C.c_void_p()
         self.ctx._check(self.lib.plp_tracker_match_counts(self._trk, C.byref(m), C.byref(l)))
-        out = {}
-        for name, p in (("motion", m), ("local", l)):
-            a = None
-            if p.value:
-                a = np.zeros(batch, np.uint32)
-                self.ctx._check(self.lib.plp_dev_download(self.ctx.handle, a.ctypes.data_as(_P), p, C.c_size_t(a.nbytes)))
-            out[name] = a
-        return out
+        return {name: self._download_ptr(p.value, np.uint32, (batch,)) if p.value else None
+                for name, p in (("motion", m), ("local", l))}
 
     def download_tracking(self, batch: int):
         self._after_tracking()
         n = self.d_n.download(np.int32, (batch,))
-        matched = self.d_matched.download(np.int32, (self.max_batch, self.cap))[:batch]
-        return dict(matched=[matched[b, :n[b]].copy() for b in range(batch)],
-                    pose=self.d_pose.download(np.float64, (batch, 4, 4)),
-                    num_valid=self.d_num_valid.download(np.int32, (batch,)),
-                    n_inliers=self.d_n_inl.download(np.int32, (batch,)),
-                    lm_iters=self.d_lm.download(np.int32, (batch,)),
-                    status=self.d_status.download(np.int32, (batch,)))
+        return dict(matched=self._keypoint_rows(n, self.d_matched), **self._tail_results(batch, self._motion_out))
