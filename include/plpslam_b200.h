@@ -972,6 +972,53 @@ PLP_API plp_status plp_tracker_updated_local_idx(const plp_tracker *t, const int
                                                  const int32_t **d_local_idx_offsets);
 
 /* ------------------------------------------------------------------------ */
+/* data::bow_database (data/bow_database.cc) on the device, scored with DBoW2::L1Scoring::score.  Keyframes are
+ * identified by their keyframe-table index (the index plp_track_map uses; fill the table in keyframe::id_ order).  The
+ * database stores one bow_vec_ per index (ascending word ids, double weights, at most max_words_per_keyframe words) and
+ * keeps an inverted index (word -> ascending keyframe indices) of its members on the device.  Membership is explicit:
+ * a keyframe that will_be_erased() but has not been erased is still a member.  An erased keyframe's vector stays
+ * stored, so it can still be scored.
+ *
+ * Candidate lists are the reference's unordered_set in one fixed order: ascending keyframe index, no duplicates.  Per
+ * query, status 0 = ok (the list may be empty), 1 = more than max_candidates (the list is left empty).  Every entry
+ * runs on the database's context and returns when its work is done (host arrays in and out), so calls on one database
+ * are ordered by the caller's thread; a database is not safe for concurrent calls from several threads.
+ * The covisibility graph is {num_keyframes, cov_offsets[num_keyframes + 1], cov_kf}: get_top_n_covisibilities(10) of
+ * every keyframe index below num_keyframes, in list order (only the first 10 entries of a longer list count); every
+ * member's index must lie below num_keyframes. */
+typedef struct plp_bow_db plp_bow_db;
+/* A database for keyframe indices [0, max_keyframes) over vocab's words.  PLP_ERR_CAPACITY, before anything is
+ * allocated, when the store or one query's count table (12 bytes per keyframe) does not fit the device. */
+PLP_API plp_status plp_bow_db_create(plp_ctx *ctx, const plp_bow_vocab *vocab, int max_keyframes,
+                                     int max_words_per_keyframe, plp_bow_db **out);
+PLP_API void plp_bow_db_destroy(plp_bow_db *db);
+/* add_keyframe of n keyframes: keyframe kf_index[i] stores word_id / weight [vec_offsets[i], vec_offsets[i + 1]) and
+ * joins the index.  PLP_ERR_INVALID, storing nothing, for an index out of range, repeated or already a member, a vector
+ * longer than max_words_per_keyframe, words not strictly ascending, or a word id outside the vocabulary.  Host arrays;
+ * runs on the database's context and returns once the index is rebuilt on the device. */
+PLP_API plp_status plp_bow_db_add_keyframes(plp_bow_db *db, int n, const int32_t *kf_index, const int32_t *vec_offsets,
+                                            const int32_t *word_id, const double *weight);
+/* erase_keyframe of n members (PLP_ERR_INVALID, nothing changed, for a non-member or a repeated index). */
+PLP_API plp_status plp_bow_db_erase_keyframes(plp_bow_db *db, int n, const int32_t *kf_index);
+/* bow_vocab_->score(bow_vec_(kf_a[i]), bow_vec_(kf_b[i])) of stored vectors, as float (host arrays). */
+PLP_API plp_status plp_bow_db_score_pairs(plp_bow_db *db, int n, const int32_t *kf_a, const int32_t *kf_b,
+                                          float *score_out);
+/* acquire_relocalization_candidates of nq query vectors (CSR of host arrays, as for add), against the members.
+ * cand_out: nq x max_candidates; num_cand_out, status_out: nq. */
+PLP_API plp_status plp_bow_db_relocalization_candidates(plp_bow_db *db, int nq, const int32_t *q_offsets,
+                                                        const int32_t *q_word_id, const double *q_weight,
+                                                        int num_keyframes, const int32_t *cov_offsets,
+                                                        const int32_t *cov_kf, int max_candidates, int32_t *cand_out,
+                                                        int32_t *num_cand_out, int32_t *status_out);
+/* acquire_loop_candidates(query_kf[q], min_score[q]) of nq stored keyframes: the query keyframe and its
+ * get_connected_keyframes() (conn_kf[conn_offsets[q] ..]) are counted but never candidates.  Whether the query keyframe
+ * is a member does not change the result, so it may be added before it is queried. */
+PLP_API plp_status plp_bow_db_loop_candidates(plp_bow_db *db, int nq, const int32_t *query_kf, const float *min_score,
+                                              const int32_t *conn_offsets, const int32_t *conn_kf, int num_keyframes,
+                                              const int32_t *cov_offsets, const int32_t *cov_kf, int max_candidates,
+                                              int32_t *cand_out, int32_t *num_cand_out, int32_t *status_out);
+
+/* ------------------------------------------------------------------------ */
 /* local bundle adjustment (optimize/local_bundle_adjuster*.cc)               */
 /* ------------------------------------------------------------------------ */
 /* The graph the reference gathers at local_bundle_adjuster.cc:72-272 (pointer-graph walk, stays in the adapter):

@@ -39,6 +39,7 @@ FILE_FLAGS = {
     "local_map.cu": NO_FMA,
     "keyframe_track.cu": NO_FMA,
     "robust_track.cu": NO_FMA,
+    "bow_db.cu": NO_FMA,
 }
 
 

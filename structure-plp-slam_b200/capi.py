@@ -790,6 +790,110 @@ def fold_bow(word_id, node_id, weight):
     return words, vals, (np.array(nodes, np.uint32), offsets, indices)
 
 
+def _csr(lists, dtype):
+    """Ragged lists -> (offsets int32[n + 1], flat dtype[max(total, 1)])."""
+    lists = [np.asarray(v, dtype).ravel() for v in lists]
+    offsets = np.zeros(len(lists) + 1, np.int32)
+    for i, v in enumerate(lists):
+        offsets[i + 1] = offsets[i] + len(v)
+    flat = np.zeros(max(int(offsets[-1]), 1), dtype)
+    if offsets[-1]:
+        flat[:offsets[-1]] = np.concatenate(lists)
+    return offsets, flat
+
+
+class BowDatabase:
+    """data::bow_database backed by plp_bow_db: keyframes are keyframe-table indices, vectors are (words, values) pairs
+    (bow_vec_: ascending word ids, double values, as fold_bow returns them).  Candidate lists come back ascending."""
+
+    def __init__(self, ctx: Context, vocab: BowVocabulary, max_keyframes: int, max_words_per_keyframe: int):
+        self._ctx = ctx
+        self._lib = ctx._lib
+        self.max_keyframes = int(max_keyframes)
+        self._h = None
+        h = C.c_void_p()
+        ctx._check(self._lib.plp_bow_db_create(ctx.handle, vocab.handle, C.c_int(max_keyframes),
+                                               C.c_int(max_words_per_keyframe), C.byref(h)))
+        self._h = h
+
+    def close(self):
+        if self._h is not None:
+            self._lib.plp_bow_db_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    @property
+    def handle(self):
+        return self._h
+
+    def add(self, kf_index, vectors):
+        """add_keyframe of keyframe kf_index[i] with bow_vec_ vectors[i] = (words, values)."""
+        kf = np.ascontiguousarray(kf_index, np.int32).ravel()
+        off, words = _csr([v[0] for v in vectors], np.int32)
+        _, vals = _csr([v[1] for v in vectors], np.float64)
+        self._ctx._check(self._lib.plp_bow_db_add_keyframes(self._h, C.c_int(len(kf)), kf.ctypes.data_as(_P),
+                                                            off.ctypes.data_as(_P), words.ctypes.data_as(_P),
+                                                            vals.ctypes.data_as(_P)))
+
+    def erase(self, kf_index):
+        kf = np.ascontiguousarray(kf_index, np.int32).ravel()
+        self._ctx._check(self._lib.plp_bow_db_erase_keyframes(self._h, C.c_int(len(kf)), kf.ctypes.data_as(_P)))
+
+    def score_pairs(self, kf_a, kf_b) -> np.ndarray:
+        a = np.ascontiguousarray(kf_a, np.int32).ravel()
+        b = np.ascontiguousarray(kf_b, np.int32).ravel()
+        out = np.zeros(max(len(a), 1), np.float32)
+        self._ctx._check(self._lib.plp_bow_db_score_pairs(self._h, C.c_int(len(a)), a.ctypes.data_as(_P),
+                                                          b.ctypes.data_as(_P), out.ctypes.data_as(_P)))
+        return out[:len(a)].copy()
+
+    @staticmethod
+    def _graph(cov):
+        """cov[k] = keyframe k's get_top_n_covisibilities(10), for every keyframe index below len(cov)."""
+        off, flat = _csr(cov, np.int32)
+        return len(cov), off, flat
+
+    def _results(self, n, max_candidates, cand, num, status):
+        lists = [cand[q, :num[q]].copy() for q in range(n)]
+        return lists, status[:n].copy()
+
+    def relocalization_candidates(self, vectors, cov, max_candidates=256):
+        """acquire_relocalization_candidates of each query vector -> (candidate lists, status per query)."""
+        n = len(vectors)
+        off, words = _csr([v[0] for v in vectors], np.int32)
+        _, vals = _csr([v[1] for v in vectors], np.float64)
+        nk, coff, ckf = self._graph(cov)
+        cand = np.zeros((max(n, 1), max(max_candidates, 1)), np.int32)
+        num = np.zeros(max(n, 1), np.int32)
+        status = np.full(max(n, 1), -1, np.int32)
+        self._ctx._check(self._lib.plp_bow_db_relocalization_candidates(
+            self._h, C.c_int(n), off.ctypes.data_as(_P), words.ctypes.data_as(_P), vals.ctypes.data_as(_P),
+            C.c_int(nk), coff.ctypes.data_as(_P), ckf.ctypes.data_as(_P), C.c_int(max_candidates),
+            cand.ctypes.data_as(_P), num.ctypes.data_as(_P), status.ctypes.data_as(_P)))
+        return self._results(n, max_candidates, cand, num, status)
+
+    def loop_candidates(self, query_kf, min_score, connected, cov, max_candidates=256):
+        """acquire_loop_candidates(query_kf[q], min_score[q]) with connected[q] = its get_connected_keyframes()."""
+        qk = np.ascontiguousarray(query_kf, np.int32).ravel()
+        n = len(qk)
+        ms = np.ascontiguousarray(np.broadcast_to(np.asarray(min_score, np.float32), (n,)))
+        conn_off, conn = _csr(connected, np.int32)
+        nk, coff, ckf = self._graph(cov)
+        cand = np.zeros((max(n, 1), max(max_candidates, 1)), np.int32)
+        num = np.zeros(max(n, 1), np.int32)
+        status = np.full(max(n, 1), -1, np.int32)
+        self._ctx._check(self._lib.plp_bow_db_loop_candidates(
+            self._h, C.c_int(n), qk.ctypes.data_as(_P), ms.ctypes.data_as(_P), conn_off.ctypes.data_as(_P),
+            conn.ctypes.data_as(_P), C.c_int(nk), coff.ctypes.data_as(_P), ckf.ctypes.data_as(_P),
+            C.c_int(max_candidates), cand.ctypes.data_as(_P), num.ctypes.data_as(_P), status.ctypes.data_as(_P)))
+        return self._results(n, max_candidates, cand, num, status)
+
+
 class OrbExtractor:
     """feature::orb_extractor (feature/orb_extractor.h:46-98) backed by plp_orb."""
 
