@@ -551,6 +551,34 @@ PLP_API plp_status plp_essential_ransac(plp_ctx *ctx, const double *bearings_1, 
                                         double *best_score_out, int32_t *solution_is_valid_out);
 
 /* ------------------------------------------------------------------------ */
+/* EPnP RANSAC  (solve/pnp_solver.{h,cc})                                    */
+/* ------------------------------------------------------------------------ */
+/* solve::pnp_solver(bearings, keypts, landmarks, scale_factors, min_num_inliers).find_via_ransac(num_iter, recompute)
+ * (solve/pnp_solver.cc:36-153) for P independent problems; problem p owns correspondences [corr_offsets[p],
+ * corr_offsets[p+1]).  relocalizer::relocalize (module/relocalizer.cc:94) runs find_via_ransac(30) once per candidate
+ * keyframe; all candidates go in one call.
+ * max_cos_error[i] is the constructor's max_cos_errors_ entry (util::cos(scale_factors[octave] * 1 degree), as float).
+ * `samples` holds, per problem, the num_iter x 4 problem-local indices the reference draws with
+ * util::create_random_array(4, 0, n - 1) (a fresh mt19937 seeded from std::random_device, so the reference's own result is
+ * not reproducible; with the samples as an input the result is a deterministic function of them).
+ * A problem with n < 4 or n < min_num_inliers does not run (:76-80): valid 0, num_inliers 0, nothing else written, its
+ * samples not read.  A problem that runs writes num_inliers (RANSAC's max_num_inliers), its n inlier flags (the first
+ * hypothesis with the most inliers wins; all 0 if no hypothesis found one) and, only when valid (num_inliers >
+ * min_num_inliers), pose_cw_out[16 p ..] = to_eigen_cam_pose(R, t) row-major -- recomputed over the inliers when
+ * `recompute` is set; the flags stay the RANSAC winner's.  There is no per-problem size limit; num_iter above 65535
+ * returns PLP_ERR_CAPACITY before anything is launched.
+ * PLP_ERR_INVALID, nothing launched: a null pointer, offsets not non-decreasing from 0, a negative size, or a sample index
+ * outside [0, n_p) in a problem that runs.  Host arrays in and out; returns when the results are written.
+ * EPnP's Eigen decompositions are restated with Jacobi rotations (csrc/pnpmath.h). */
+PLP_API plp_status plp_pnp_ransac(plp_ctx *ctx, int num_problems, const int32_t *corr_offsets,
+                                  const double *bearings /* N x 3 */, const double *pos_w /* N x 3 */,
+                                  const float *max_cos_error /* N */,
+                                  const int32_t *samples /* P x num_iter x 4, problem-local */, int num_iter,
+                                  int min_num_inliers, int recompute, int32_t *valid_out /* P */,
+                                  int32_t *num_inliers_out /* P */, double *pose_cw_out /* P x 16 */,
+                                  uint8_t *is_inlier_out /* N */);
+
+/* ------------------------------------------------------------------------ */
 /* plane RANSAC  (planar_mapping_module.{h,cc})                              */
 /* ------------------------------------------------------------------------ */
 /* Planar_Mapping_module::estimate_plane_sequential_RANSAC (planar_mapping_module.cc:412-591, mode 0) and

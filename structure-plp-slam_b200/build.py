@@ -40,6 +40,7 @@ FILE_FLAGS = {
     "keyframe_track.cu": NO_FMA,
     "robust_track.cu": NO_FMA,
     "bow_db.cu": NO_FMA,
+    "pnp.cu": NO_FMA,
 }
 
 

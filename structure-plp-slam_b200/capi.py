@@ -495,6 +495,28 @@ class Context:
             inl.ctypes.data_as(_P), E.ctypes.data_as(_P), C.byref(score), C.byref(valid)))
         return int(valid.value), inl[:len(m)].copy(), E.reshape(3, 3), float(score.value)
 
+    # ------------------------------------------------------------------ solve::pnp_solver
+    def pnp_ransac(self, corr_offsets, bearings, pos_w, max_cos_error, samples, min_num_inliers=10, recompute=True):
+        """solve::pnp_solver::find_via_ransac of P problems in one call (plp_pnp_ransac).  corr_offsets: P + 1; bearings,
+        pos_w: N x 3; max_cos_error: N float; samples: P x num_iter x 4 problem-local indices.  Returns (valid (P),
+        num_inliers (P), pose_cw (P x 4 x 4, NaN where not written), is_inlier (N, 255 where not written))."""
+        off = np.ascontiguousarray(corr_offsets, np.int32)
+        P = len(off) - 1
+        N = int(off[-1]) if P >= 0 and len(off) else 0
+        k = _Keep()
+        sm = np.ascontiguousarray(samples, np.int32)
+        num_iter = int(sm.shape[1]) if sm.ndim == 3 else 0
+        valid = np.zeros(max(P, 1), np.int32)
+        num = np.zeros(max(P, 1), np.int32)
+        pose = np.full((max(P, 1), 16), np.nan)
+        flags = np.full(max(N, 1), 255, np.uint8)
+        self._check(self._lib.plp_pnp_ransac(
+            self._h, C.c_int(P), k.arr(off, np.int32), k.arr(np.reshape(bearings, -1), np.float64),
+            k.arr(np.reshape(pos_w, -1), np.float64), k.arr(max_cos_error, np.float32), k.arr(sm.reshape(-1), np.int32),
+            C.c_int(num_iter), C.c_int(min_num_inliers), C.c_int(1 if recompute else 0), valid.ctypes.data_as(_P),
+            num.ctypes.data_as(_P), pose.ctypes.data_as(_P), flags.ctypes.data_as(_P)))
+        return valid[:P].copy(), num[:P].copy(), pose[:P].reshape(P, 4, 4).copy(), flags[:N].copy()
+
     # ------------------------------------------------------------------ Planar_Mapping_module
     def plane_ransac(self, pos_w, valid, samples, cfg, eq0=(0, 0, 0, 0), err0=0.0):
         """estimate_plane_sequential_RANSAC (cfg['mode'] = 0) / update_plane_via_RANSAC (1) with caller-drawn index samples

@@ -42,6 +42,7 @@
 #include <random>
 #include "PLPSLAM/data/map_database.h"
 #include "PLPSLAM/data/graph_node.h"
+#include "PLPSLAM/util/trigonometric.h"
 #include "plpslam_b200.h"
 #include "plpslam_b200_line_trimming.h"
 
@@ -439,6 +440,70 @@ inline unsigned robust_match_frame_and_keyframe(PLPSLAM::data::frame &frm, PLPSL
         ++num_inlier_matches;
     }
     return num_inlier_matches;
+}
+
+// ---- relocalizer::relocalize's EPnP (module/relocalizer.cc:86-100) for every candidate keyframe in one call ----------
+// run[i]: the candidate reached the loop's pnp_solver (not will_be_erased(), >= min_num_bow_matches_ BoW matches).  The
+// correspondences are extract_valid_indices / setup_pnp_solver's (:254-291); max_cos_error and the 4-point samples are
+// computed with the reference's own util::cos and util::create_random_array, and samples are drawn only for candidates
+// that run.  Result i stands in for pnp_solver i: valid, get_best_cam_pose(), and
+// resample_by_indices(valid_indices, get_inlier_flags()) (frame keypoint indices).
+struct pnp_candidate_result {
+    bool valid = false;
+    PLPSLAM::Mat44_t pose_cw;
+    std::vector<unsigned> inlier_indices;
+};
+
+inline std::vector<pnp_candidate_result> pnp_ransac_candidates(const PLPSLAM::data::frame &curr_frm,
+                                                               const std::vector<std::vector<PLPSLAM::data::landmark *>> &matched_landmarks,
+                                                               const std::vector<bool> &run, unsigned num_iter = 30,
+                                                               unsigned min_num_inliers = 10) {
+    const size_t K = matched_landmarks.size();
+    if (run.size() != K) throw std::invalid_argument("plpslam_b200::pnp_ransac_candidates: run and matched_landmarks differ in size");
+    constexpr double max_rad_error = 1.0 * M_PI / 180.0;  // pnp_solver.cc:47
+    std::vector<int32_t> off(K + 1, 0), samples;
+    std::vector<std::vector<unsigned>> valid_indices(K);
+    std::vector<double> bearings, pos_w;
+    std::vector<float> max_cos;
+    for (size_t k = 0; k < K; ++k) {
+        if (run[k]) {
+            for (unsigned idx = 0; idx < matched_landmarks[k].size(); ++idx) {
+                auto *lm = matched_landmarks[k][idx];
+                if (!lm || lm->will_be_erased()) continue;
+                valid_indices[k].push_back(idx);
+                const PLPSLAM::Vec3_t pw = lm->get_pos_in_world();
+                for (int c = 0; c < 3; ++c) bearings.push_back(curr_frm.bearings_[idx](c)), pos_w.push_back(pw(c));
+                max_cos.push_back(PLPSLAM::util::cos(curr_frm.scale_factors_.at(curr_frm.keypts_[idx].octave) * max_rad_error));
+            }
+        }
+        const unsigned n = (unsigned)valid_indices[k].size();
+        off[k + 1] = off[k] + (int32_t)n;
+        for (unsigned it = 0; it < num_iter; ++it) {
+            if (n >= 4 && n >= min_num_inliers) {
+                const auto idx = PLPSLAM::util::create_random_array(4, 0U, n - 1);
+                samples.insert(samples.end(), idx.begin(), idx.end());
+            } else {
+                samples.insert(samples.end(), 4, 0);  // not read: the problem does not run
+            }
+        }
+    }
+    const size_t N = (size_t)off[K];
+    std::vector<int32_t> valid(K), num_inliers(K);
+    std::vector<double> pose(K * 16);
+    std::vector<uint8_t> flags(N + 1);
+    check(plp_pnp_ransac(thread_ctx(), (int)K, off.data(), bearings.data(), pos_w.data(), max_cos.data(), samples.data(),
+                         (int)num_iter, (int)min_num_inliers, /*recompute=*/1, valid.data(), num_inliers.data(), pose.data(),
+                         flags.data()));
+    std::vector<pnp_candidate_result> out(K);
+    for (size_t k = 0; k < K; ++k) {
+        out[k].valid = run[k] && valid[k];
+        if (!out[k].valid) continue;
+        for (int r = 0; r < 4; ++r)
+            for (int c = 0; c < 4; ++c) out[k].pose_cw(r, c) = pose[16 * k + 4 * r + c];
+        for (size_t i = 0; i < valid_indices[k].size(); ++i)
+            if (flags[off[k] + i]) out[k].inlier_indices.push_back(valid_indices[k][i]);
+    }
+    return out;
 }
 
 // ---- match::fuse::replace_duplication (match/fuse.cc:153-300) over the loop of mapping_module.cc:711-714 / :749 ---

@@ -79,11 +79,24 @@ def rectify():
     np.savez_compressed(OUT / "cv2_rectify.npz", **out)
 
 
+def cv2_epnp():
+    """cv2.solvePnP(..., SOLVEPNP_EPNP) with K = I on non-minimal noisy inlier sets of tests/pnp_data.py's scenes."""
+    import pnp_data
+    out = {}
+    for i, (seed, n) in enumerate([(1, 6), (2, 10), (3, 30), (4, 100), (5, 300), (6, 1000)]):
+        s = pnp_data.make_scene(500 + seed, n, 0.0, noise_px=0.5)
+        uv = s["bearings"][:, :2] / s["bearings"][:, 2:3]
+        _, rv, tv = cv2.solvePnP(s["pos_w"], uv, np.eye(3), None, flags=cv2.SOLVEPNP_EPNP)
+        out[f"bearings_{i}"], out[f"pos_w_{i}"] = s["bearings"], s["pos_w"]
+        out[f"R_{i}"], out[f"t_{i}"] = cv2.Rodrigues(rv)[0], tv.ravel()
+    np.savez_compressed(OUT / "cv2_epnp.npz", cv2_version=np.array(cv2.__version__), **out)
+
+
 def main():
     OUT.mkdir(exist_ok=True)
     if sys.argv[1:]:
         for name in sys.argv[1:]:
-            {"cv2_lsd_odd": lsd_odd, "cv2_undistort": undistort, "cv2_rectify": rectify}[name]()
+            {"cv2_lsd_odd": lsd_odd, "cv2_undistort": undistort, "cv2_rectify": rectify, "cv2_epnp": cv2_epnp}[name]()
         return
     orc = oracle_api.Oracle()
     tex = synth.make_texture(4321, 240, 320, n_rect=120, n_blob=500)      # the image of __graft_entry__.smoke()
@@ -122,6 +135,7 @@ def main():
     lsd_odd()
     undistort()
     rectify()
+    cv2_epnp()
     for f in sorted(OUT.glob("*.npz")):
         print(f.name, f.stat().st_size, "bytes")
 
