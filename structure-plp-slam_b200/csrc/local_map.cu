@@ -50,6 +50,7 @@ plp_status plp_tracker_reserve_local_map(plp_tracker *t, float log_scale_factor,
     L.out(D->qx, B * ML);
     L.out(D->qy, B * ML);
     L.out(D->qradius, B * ML);
+    if (t->stereo()) L.out(D->qxr, B * ML);
     L.out(D->qmin, B * ML);
     L.out(D->qmax, B * ML);
     L.out(D->qvalid, B * ML);
@@ -102,6 +103,7 @@ plp_status plp_tracker_local_map_track_batch_dev(plp_tracker *t, int batch, cons
     D.x = M.x;
     D.y = M.y;
     D.octave = M.octave;
+    D.x_right = M.x_right;
     D.desc = M.desc;
     for (int l = 0; l < 16; ++l) D.inv_level_sigma_sq[l] = t->tail[kStageMotion].inv_level_sigma_sq[l];
     D.motion = t->record[kStageMotion];

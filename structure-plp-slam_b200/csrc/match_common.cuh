@@ -226,4 +226,36 @@ __device__ __forceinline__ Reproj reproject(const plp_camera &cam, const double 
     return r;
 }
 
+// ---- projection.cc:220-238: the forward / backward motion assumption of match_current_and_last_frames, from the 4 x 4
+// row-major poses of the current and last frames.  One copy for the host entry points (match.cu) and the batched
+// motion stage (pipeline.cu).  The device products and sums are explicitly rounded, so the flags equal the oracle's in
+// every translation unit, whatever its -fmad setting.
+__host__ __device__ __forceinline__ double mul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dmul_rn(a, b);
+#else
+    return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ double add_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+    return __dadd_rn(a, b);
+#else
+    return a + b;
+#endif
+}
+
+__host__ __device__ __forceinline__ void motion_assumption(const plp_camera &cam, const double *Tc, const double *Tl,
+                                                           int *fwd, int *bwd) {
+    // trans_wc = -R_cw^T t_cw ; trans_lc = R_lw trans_wc + t_lw
+    double twc[3];
+    for (int r = 0; r < 3; ++r)
+        twc[r] = -add_rn(add_rn(mul_rn(Tc[0 * 4 + r], Tc[3]), mul_rn(Tc[1 * 4 + r], Tc[7])), mul_rn(Tc[2 * 4 + r], Tc[11]));
+    const double tlc_z =
+        add_rn(add_rn(add_rn(mul_rn(Tl[8], twc[0]), mul_rn(Tl[9], twc[1])), mul_rn(Tl[10], twc[2])), Tl[11]);
+    const bool mono = cam.setup_type == 0;
+    *fwd = mono ? 0 : (tlc_z > cam.true_baseline);
+    *bwd = mono ? 0 : (-tlc_z > cam.true_baseline);
+}
+
 }  // namespace plp

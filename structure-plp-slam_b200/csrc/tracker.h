@@ -33,6 +33,7 @@ struct TrackDev {
     const plp_keypoint *kp;
     const uint8_t *desc;
     const int32_t *n_kp;
+    const float *x_right;    // batch x cap: stereo_x_right_ (stereo trackers; null for monocular)
     // last frames
     const double *last_pos_w;
     const int32_t *last_octave;
@@ -122,6 +123,9 @@ struct plp_tracker {
     plp::UndistJob undist;             // camera and coefficients; kp / n_kp / batch set per call
     plp_keypoint *d_undist = nullptr;  // max_batch x cap (inside d_block)
     double *d_bearings = nullptr;      // max_batch x cap x 3
+    // a stereo tracker's current-frame stereo_x_right_ (plp_tracker_bind_stereo): max_batch x cap, caller-owned
+    const float *d_x_right = nullptr;
+    bool stereo() const { return cam.setup_type == 1; }
     // the most recent motion_track_batch_dev: its inputs and scratch, which the later stages read
     plp::TrackDev motion;
     // per stage: its tail job with the scratch bound (at create or reserve), and the record its most recent call left;
@@ -145,6 +149,7 @@ struct plp_tracker {
     // ran on it, so a keyframe or robust record that stands must cover the batch too.
     plp_status check_order(int s, int batch) const {
         PLP_REQUIRE(batch >= 1 && batch <= max_batch, "batch exceeds the tracker's max_batch");
+        PLP_REQUIRE(!stereo() || d_x_right, "a stereo tracker needs plp_tracker_bind_stereo first");
         if (s == plp::kStageRobust)
             PLP_REQUIRE(covers(plp::kStageKeyframe, batch),
                         "the batch must follow a plp_tracker_keyframe_track_batch_dev of at least as many frames");
@@ -170,6 +175,7 @@ struct plp_tracker {
         J.x = motion.x;
         J.y = motion.y;
         J.octave = motion.octave;
+        J.x_right = motion.x_right;
         J.matched = matched;
         J.pose = pose;
         J.num_valid = num_valid;

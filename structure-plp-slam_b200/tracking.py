@@ -1,5 +1,5 @@
-"""Device-resident batched front-end: ORB extraction + motion-based tracking (+ optionally the keyframe and robust
-trackers and the local-map stage) without leaving HBM.
+"""Device-resident batched front-end: ORB extraction (+ the right image's and match::stereo::compute for a stereo camera)
++ motion-based tracking (+ optionally the keyframe and robust trackers and the local-map stage) without leaving HBM.
 
 Thin ctypes layer over plp_orb_extract_batch_dev + plp_tracker_motion_track_batch_dev (+
 plp_tracker_keyframe_track_batch_dev, plp_tracker_robust_track_batch_dev, plp_tracker_update_local_map_batch_dev,
@@ -146,12 +146,15 @@ class FrontEnd:
 
     def __init__(self, ctx: Context, rows: int, cols: int, cam, max_batch: int, max_last_points: int = 4096,
                  max_num_keypts=1000, scale_factor=1.2, num_levels=8, ini_fast_thr=20, min_fast_thr=7,
-                 track_ctx: Context | None = None, distortion=None):
+                 track_ctx: Context | None = None, distortion=None, right_ctx: Context | None = None):
         """track_ctx: optional second context (stream) for the tracking kernels; extraction stays on `ctx`.  The two
         streams are chained by plp_ctx_wait_ctx, so extract(k + 1) of ANOTHER FrontEnd can run under track(k).
         distortion: a capi.Distortion (make_distortion); the tracker then undistorts the keypoints before matching, and
         cam's bounds and the grid come from the undistorted image corners (capi.make_distorted_camera).  None: the
-        camera has no distortion."""
+        camera has no distortion.
+        A stereo camera (cam.setup_type 1, rectified pairs) adds a second extractor for the right images and the
+        stereo_x_right_ / depths_ buffers that extract() fills with match::stereo::compute; the tracker reads x_right.
+        right_ctx: optional context (stream) for the right image's ORB pass, which then runs beside the left one."""
         self.ctx = ctx
         self.track_ctx = track_ctx if track_ctx is not None else ctx
         self.lib = ctx._lib
@@ -174,6 +177,18 @@ class FrontEnd:
                                                   C.c_int(max_batch), C.c_int(self.cap), C.c_int(max_last_points),
                                                   None if distortion is None else C.byref(distortion), C.byref(h)))
         self._trk = h
+        self.stereo = cam.setup_type == 1
+        self.orb_right = None
+        self._stereo_out = None
+        if self.stereo:
+            self.right_ctx = right_ctx if right_ctx is not None else ctx
+            self.orb_right = OrbExtractor(self.right_ctx, rows, cols, max_num_keypts, scale_factor, num_levels,
+                                          ini_fast_thr, min_fast_thr, max_batch=max_batch)
+            self._stereo_out = self._frame_buffers(imgs_right=rows * cols, kp_right=self.cap * KP_DTYPE.itemsize,
+                                                   desc_right=self.cap * 32, n_kp_right=4, status_right=4,
+                                                   x_right=self.cap * 4, depths=self.cap * 4)
+            self.d_x_right = self._stereo_out["x_right"]
+            ctx._check(self.lib.plp_tracker_bind_stereo(self._trk, self.d_x_right.ptr))
         self._motion_out = self._frame_buffers(imgs=rows * cols, kp=self.cap * KP_DTYPE.itemsize, desc=self.cap * 32,
                                                n_kp=4, status=4, matched=self.cap * 4, pose=128, num_valid=4,
                                                n_inliers=4, lm_iters=4)
@@ -206,7 +221,8 @@ class FrontEnd:
     def close(self):
         """Frees the tracker and every device and pinned buffer this FrontEnd still holds; a buffer a caller has taken
         out of its hands (by replacing the attribute) is the caller's.  A second call does nothing."""
-        outs = [o for o in (self._motion_out, self._local_out, self._kf_out, self._rb_out, self._upd_out) if o]
+        outs = [o for o in (self._motion_out, self._local_out, self._kf_out, self._rb_out, self._upd_out,
+                            self._stereo_out) if o]
         for b in ([b for o in outs for b in o.values()] + self._last_bufs + self._last_pinned + self._local_bufs +
                   self._kf_bufs + self._map_bufs + [self._pin_imgs, self._pin_out]):
             if b is not None:
@@ -215,10 +231,18 @@ class FrontEnd:
             self.lib.plp_tracker_destroy(self._trk)
             self._trk = None
         self.orb.close()
+        if self.orb_right is not None:
+            self.orb_right.close()
+            self.orb_right = None
 
     # -- inputs ---------------------------------------------------------------------------------------
-    def upload_images(self, imgs: np.ndarray):
+    def upload_images(self, imgs: np.ndarray, right: np.ndarray | None = None):
+        """imgs: the (left) images; right: the right images of a stereo FrontEnd, required there."""
+        if self.stereo != (right is not None):
+            raise PlpError("a stereo FrontEnd takes left and right images, a monocular one left images only")
         self.d_imgs.upload(np.ascontiguousarray(imgs, np.uint8))
+        if right is not None:
+            self._stereo_out["imgs_right"].upload(np.ascontiguousarray(right, np.uint8))
 
     def set_last_frames(self, last_list, pose_pred, pose_last):
         """last_list[b]: dict(pos_w[m,3], octave[m], angle[m], desc[m,32], valid[m]|None)."""
@@ -408,9 +432,24 @@ class FrontEnd:
     def extract(self, batch: int):
         if self.track_ctx is not self.ctx:
             self.ctx.wait(self.track_ctx)  # the previous track() still reads the keypoint / descriptor arrays
+        if self.stereo:  # frame.cc:456-457: the right image's ORB pass
+            o, rc = self._stereo_out, self.right_ctx
+            if rc is not self.ctx:
+                rc.wait(self.ctx)  # the previous stereo match still reads the right keypoints and pyramid
+            rc._check(self.lib.plp_orb_extract_batch_dev(self.orb_right.handle, o["imgs_right"].ptr, C.c_int(batch),
+                                                         C.c_size_t(self.cols), o["kp_right"].ptr, o["desc_right"].ptr,
+                                                         o["n_kp_right"].ptr, o["status_right"].ptr))
         self.ctx._check(self.lib.plp_orb_extract_batch_dev(self.orb.handle, self.d_imgs.ptr, C.c_int(batch),
                                                           C.c_size_t(self.cols), self.d_kp.ptr, self.d_desc.ptr,
                                                           self.d_n.ptr, self.d_status.ptr))
+        if self.stereo:  # frame.cc:470-480: stereo_x_right_ and depths_ of the left keypoints
+            if rc is not self.ctx:
+                self.ctx.wait(rc)
+            self.ctx._check(self.lib.plp_stereo_compute_batch_dev(
+                self.ctx.handle, self.orb.handle, self.orb_right.handle, C.c_int(batch), self.d_kp.ptr,
+                self.d_desc.ptr, self.d_n.ptr, o["kp_right"].ptr, o["desc_right"].ptr, o["n_kp_right"].ptr,
+                C.c_float(self.cam.focal_x_baseline), C.c_float(self.cam.true_baseline), o["x_right"].ptr,
+                o["depths"].ptr, None))
 
     def track(self, batch: int, margin: float = 20.0):
         if self.track_ctx is not self.ctx:
@@ -511,6 +550,16 @@ class FrontEnd:
         n = self.d_n.download(np.int32, (batch,))
         return list(zip(self._keypoint_rows(n, self.d_kp, KP_DTYPE),
                         _by_frame(n, self.d_desc.download(np.uint8, (self.max_batch, self.cap, 32)))))
+
+    def download_stereo(self, batch: int):
+        """Per frame (stereo_x_right_, depths_) of the last extract() of a stereo FrontEnd, one entry per left
+        keypoint (-1: no stereo match)."""
+        if not self.stereo:
+            raise PlpError("FrontEnd without a stereo camera")
+        self._after_tracking()
+        n = self.d_n.download(np.int32, (batch,))
+        return list(zip(self._keypoint_rows(n, self.d_x_right, np.float32),
+                        self._keypoint_rows(n, self._stereo_out["depths"], np.float32)))
 
     def download_undistorted(self, batch: int):
         """Per frame (undistorted keypoints, bearings) of the last track() -- frame::undist_keypts_ and bearings_.
