@@ -579,6 +579,40 @@ PLP_API plp_status plp_pnp_ransac(plp_ctx *ctx, int num_problems, const int32_t 
                                   uint8_t *is_inlier_out /* N */);
 
 /* ------------------------------------------------------------------------ */
+/* Sim3 RANSAC  (solve/sim3_solver.{h,cc})                                   */
+/* ------------------------------------------------------------------------ */
+/* solve::sim3_solver(keyfrm_1, keyfrm_2, matched_lms_in_keyfrm_2, fix_scale, min_num_inliers).find_via_ransac(num_iter)
+ * (solve/sim3_solver.cc:40-191) for P independent problems; problem p owns correspondences [corr_offsets[p],
+ * corr_offsets[p+1]): the constructor's common_pts_in_keyfrm_1_ / _2_ (each landmark in its keyframe's camera frame) and
+ * chi_sq_x_sigma_sq_1_ / _2_ (the float 9.21034f * level_sigma_sq_[octave]) of :96-112.
+ * loop_detector::select_loop_candidate_via_Sim3 (module/loop_detector.cc:368-369) runs find_via_ransac(200) once per loop
+ * candidate; all candidates (or the candidates of many query keyframes) go in one call.
+ * cams[p]: the camera of both keyframes of problem p; reproject_to_image reads fx, fy, cx, cy only (the perspective and
+ * fisheye models share that formula).  fix_scale: the reference's setup_type != Monocular (system.cc:140).
+ * `samples` holds, per problem, the num_iter x 3 problem-local indices the reference draws with
+ * util::create_random_array(3, 0, n - 1) (a freshly seeded mt19937, so the reference's own result is not reproducible;
+ * with the samples as an input the result is a deterministic function of them).  Duplicate indices are legal.
+ * Every output of every problem is written.  A problem with n < 3 or n < min_num_inliers does not run (:130-134): valid 0,
+ * num_inliers 0, zero rotation / translation / scale, its samples not read.  A problem that runs writes num_inliers
+ * (RANSAC's max_num_inliers; the first hypothesis with the most inliers wins), valid = (num_inliers >= min_num_inliers)
+ * (:177) and, when valid, the winner's rot_12 (row-major), trans_12 and scale_12 (get_best_rotation_12 / translation_12 /
+ * scale_12); when invalid, the reference's zeros (:181-183).  There is no per-problem size limit; num_iter above 65535
+ * returns PLP_ERR_CAPACITY before anything is launched.
+ * PLP_ERR_INVALID, nothing launched and nothing written: a null pointer, offsets not non-decreasing from 0, a negative
+ * size, or a sample index outside [0, n_p) in a problem that runs.  Host arrays in and out; returns when the results are
+ * written.  Eigen's EigenSolver is restated with Jacobi rotations, and a point behind a camera reprojects to NaN where the
+ * reference reads an uninitialised value (csrc/sim3math.h). */
+PLP_API plp_status plp_sim3_ransac(plp_ctx *ctx, int num_problems, const int32_t *corr_offsets /* P + 1 */,
+                                   const plp_camera *cams /* P: fx, fy, cx, cy read */,
+                                   const double *pts_1 /* N x 3, keyframe-1 camera frame */,
+                                   const double *pts_2 /* N x 3, keyframe-2 camera frame */,
+                                   const float *chi_sq_1 /* N */, const float *chi_sq_2 /* N */,
+                                   const int32_t *samples /* P x num_iter x 3, problem-local */, int num_iter,
+                                   int fix_scale, int min_num_inliers, int32_t *valid_out /* P */,
+                                   int32_t *num_inliers_out /* P */, double *rot_12_out /* P x 9, row-major */,
+                                   double *trans_12_out /* P x 3 */, float *scale_12_out /* P */);
+
+/* ------------------------------------------------------------------------ */
 /* plane RANSAC  (planar_mapping_module.{h,cc})                              */
 /* ------------------------------------------------------------------------ */
 /* Planar_Mapping_module::estimate_plane_sequential_RANSAC (planar_mapping_module.cc:412-591, mode 0) and

@@ -41,6 +41,7 @@ FILE_FLAGS = {
     "robust_track.cu": NO_FMA,
     "bow_db.cu": NO_FMA,
     "pnp.cu": NO_FMA,
+    "sim3.cu": NO_FMA,
 }
 
 

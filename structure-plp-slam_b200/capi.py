@@ -517,6 +517,34 @@ class Context:
             num.ctypes.data_as(_P), pose.ctypes.data_as(_P), flags.ctypes.data_as(_P)))
         return valid[:P].copy(), num[:P].copy(), pose[:P].reshape(P, 4, 4).copy(), flags[:N].copy()
 
+    # ------------------------------------------------------------------ solve::sim3_solver
+    def sim3_ransac(self, corr_offsets, cams, pts_1, pts_2, chi_sq_1, chi_sq_2, samples, fix_scale=False,
+                    min_num_inliers=20):
+        """solve::sim3_solver::find_via_ransac of P problems in one call (plp_sim3_ransac).  corr_offsets: P + 1; cams: P
+        Camera structs (fx, fy, cx, cy read); pts_1, pts_2: N x 3 camera-frame points; chi_sq_1, chi_sq_2: N float;
+        samples: P x num_iter x 3 problem-local indices.  Returns (valid (P), num_inliers (P), rot_12 (P x 3 x 3),
+        trans_12 (P x 3), scale_12 (P, float32))."""
+        off = np.ascontiguousarray(corr_offsets, np.int32)
+        P = len(off) - 1
+        if len(cams) != P:
+            raise PlpError(f"sim3_ransac: {len(cams)} cameras for {P} problems")
+        k = _Keep()
+        cam_arr = (Camera * max(P, 1))(*cams)
+        sm = np.ascontiguousarray(samples, np.int32)
+        num_iter = int(sm.shape[1]) if sm.ndim == 3 else 0
+        valid = np.zeros(max(P, 1), np.int32)
+        num = np.zeros(max(P, 1), np.int32)
+        rot = np.zeros((max(P, 1), 9))
+        trans = np.zeros((max(P, 1), 3))
+        scale = np.zeros(max(P, 1), np.float32)
+        self._check(self._lib.plp_sim3_ransac(
+            self._h, C.c_int(P), k.arr(off, np.int32), cam_arr, k.arr(np.reshape(pts_1, -1), np.float64),
+            k.arr(np.reshape(pts_2, -1), np.float64), k.arr(chi_sq_1, np.float32), k.arr(chi_sq_2, np.float32),
+            k.arr(sm.reshape(-1), np.int32), C.c_int(num_iter), C.c_int(1 if fix_scale else 0), C.c_int(min_num_inliers),
+            valid.ctypes.data_as(_P), num.ctypes.data_as(_P), rot.ctypes.data_as(_P), trans.ctypes.data_as(_P),
+            scale.ctypes.data_as(_P)))
+        return valid[:P].copy(), num[:P].copy(), rot[:P].reshape(P, 3, 3).copy(), trans[:P].copy(), scale[:P].copy()
+
     # ------------------------------------------------------------------ Planar_Mapping_module
     def plane_ransac(self, pos_w, valid, samples, cfg, eq0=(0, 0, 0, 0), err0=0.0):
         """estimate_plane_sequential_RANSAC (cfg['mode'] = 0) / update_plane_via_RANSAC (1) with caller-drawn index samples

@@ -506,6 +506,97 @@ inline std::vector<pnp_candidate_result> pnp_ransac_candidates(const PLPSLAM::da
     return out;
 }
 
+// ---- loop_detector::select_loop_candidate_via_Sim3's linear Sim3 (module/loop_detector.cc:368-374) for every candidate in
+// one call ----
+// run[i]: candidate i reached the loop's sim3_solver (not will_be_erased(), >= 20 BoW matches); matched_lms[i] is its
+// curr_match_lms_observed_in_cand (indexed by cur_keyfrm's keypoints).  Each candidate's correspondences are the
+// sim3_solver constructor's (solve/sim3_solver.cc:46-115): camera-frame points of both keyframes and the float
+// chi_sq_2D * level_sigma_sq_[octave] of each undistorted keypoint (level_sigma_sq_ read as the bit-identical square of
+// scale_factors_, and get_index_in_keyframe as a lookup in get_observations(), so the header needs no other members).  The 3-point samples are drawn with the reference's
+// util::create_random_array, only for candidates that run.  cam: undistort_keypoints' convention (camera_of() for a
+// perspective camera, the fisheye camera's own fx_ .. cy_); fix_scale: setup_type_ != Monocular (system.cc:140).
+// Result i stands in for sim3_solver i after find_via_ransac(num_iter): solution_is_valid(), get_best_rotation_12(),
+// get_best_translation_12(), get_best_scale_12().
+struct sim3_candidate_result {
+    bool valid = false;
+    PLPSLAM::Mat33_t rot_12;
+    PLPSLAM::Vec3_t trans_12;
+    float scale_12 = 0.0f;
+};
+
+inline std::vector<sim3_candidate_result> sim3_ransac_candidates(PLPSLAM::data::keyframe *cur_keyfrm,
+                                                                 const std::vector<PLPSLAM::data::keyframe *> &candidates,
+                                                                 const std::vector<std::vector<PLPSLAM::data::landmark *>> &matched_lms,
+                                                                 const std::vector<bool> &run, bool fix_scale,
+                                                                 const plp_camera &cam, unsigned num_iter = 200,
+                                                                 unsigned min_num_inliers = 20) {
+    const size_t K = candidates.size();
+    if (matched_lms.size() != K || run.size() != K)
+        throw std::invalid_argument("plpslam_b200::sim3_ransac_candidates: candidates, matched_lms and run differ in size");
+    constexpr float chi_sq_2D = 9.21034;  // sim3_solver.cc:67
+    const auto keyfrm_1_lms = cur_keyfrm->get_landmarks();
+    const PLPSLAM::Mat33_t rot_1w = cur_keyfrm->get_rotation();
+    const PLPSLAM::Vec3_t trans_1w = cur_keyfrm->get_translation();
+    std::vector<int32_t> off(K + 1, 0), samples;
+    std::vector<double> pts_1, pts_2;
+    std::vector<float> chi_sq_1, chi_sq_2;
+    for (size_t k = 0; k < K; ++k) {
+        unsigned n = 0;
+        if (run[k]) {
+            auto *keyfrm_2 = candidates[k];
+            const PLPSLAM::Mat33_t rot_2w = keyfrm_2->get_rotation();
+            const PLPSLAM::Vec3_t trans_2w = keyfrm_2->get_translation();
+            for (unsigned idx1 = 0; idx1 < keyfrm_1_lms.size(); ++idx1) {  // :70-115
+                auto *lm_2 = matched_lms[k].at(idx1);
+                auto *lm_1 = keyfrm_1_lms.at(idx1);
+                if (!lm_1 || !lm_2) continue;
+                if (lm_1->will_be_erased() || lm_2->will_be_erased()) continue;
+                // get_index_in_keyframe(keyfrm_2) (data/landmark.cc:156-167): the observation index, or -1
+                const auto obs_2 = lm_2->get_observations();
+                const auto found = obs_2.find(keyfrm_2);
+                if (found == obs_2.end()) continue;
+                const auto &keypt_1 = cur_keyfrm->undist_keypts_.at(idx1);
+                const auto &keypt_2 = keyfrm_2->undist_keypts_.at(found->second);
+                // level_sigma_sq_[octave] == scale_factors_[octave]^2 in float: calc_level_sigma_sq squares the same
+                // float recurrence calc_scale_factors stores (feature/orb_params.cc:86-116)
+                const float sf_1 = cur_keyfrm->scale_factors_.at(keypt_1.octave);
+                const float sf_2 = keyfrm_2->scale_factors_.at(keypt_2.octave);
+                chi_sq_1.push_back(chi_sq_2D * (sf_1 * sf_1));
+                chi_sq_2.push_back(chi_sq_2D * (sf_2 * sf_2));
+                const PLPSLAM::Vec3_t p1 = rot_1w * lm_1->get_pos_in_world(), p2 = rot_2w * lm_2->get_pos_in_world();
+                for (int c = 0; c < 3; ++c) pts_1.push_back(p1(c) + trans_1w(c)), pts_2.push_back(p2(c) + trans_2w(c));
+                ++n;
+            }
+        }
+        off[k + 1] = off[k] + (int32_t)n;
+        for (unsigned it = 0; it < num_iter; ++it) {
+            if (n >= 3 && n >= min_num_inliers) {  // :130, :149
+                const auto idx = PLPSLAM::util::create_random_array(3, 0, static_cast<int>(n - 1));
+                samples.insert(samples.end(), idx.begin(), idx.end());
+            } else {
+                samples.insert(samples.end(), 3, 0);  // not read: the problem does not run
+            }
+        }
+    }
+    const std::vector<plp_camera> cams(K, cam);
+    std::vector<int32_t> valid(K), num_inliers(K);
+    std::vector<double> rot(K * 9), trans(K * 3);
+    std::vector<float> scale(K);
+    check(plp_sim3_ransac(thread_ctx(), (int)K, off.data(), cams.data(), pts_1.data(), pts_2.data(), chi_sq_1.data(),
+                          chi_sq_2.data(), samples.data(), (int)num_iter, fix_scale ? 1 : 0, (int)min_num_inliers,
+                          valid.data(), num_inliers.data(), rot.data(), trans.data(), scale.data()));
+    std::vector<sim3_candidate_result> out(K);
+    for (size_t k = 0; k < K; ++k) {
+        out[k].valid = run[k] && valid[k];
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) out[k].rot_12(r, c) = rot[9 * k + 3 * r + c];
+            out[k].trans_12(r) = trans[3 * k + r];
+        }
+        out[k].scale_12 = scale[k];
+    }
+    return out;
+}
+
 // ---- match::fuse::replace_duplication (match/fuse.cc:153-300) over the loop of mapping_module.cc:711-714 / :749 ---
 // One batched search for (targets x landmarks); the effects are applied in the reference's order.  landmark::replace
 // recomputes the surviving landmark's descriptor (data/landmark.cc:429), so a landmark whose descriptor changed is
