@@ -613,6 +613,46 @@ PLP_API plp_status plp_sim3_ransac(plp_ctx *ctx, int num_problems, const int32_t
                                    double *trans_12_out /* P x 3 */, float *scale_12_out /* P */);
 
 /* ------------------------------------------------------------------------ */
+/* Sim3 optimiser  (optimize/transform_optimizer.{h,cc})                     */
+/* ------------------------------------------------------------------------ */
+/* optimize::transform_optimizer(fix_scale, num_iter).optimize(keyfrm_1, keyfrm_2, matched_lms_in_keyfrm_2, Sim3_12, chi_sq)
+ * (optimize/transform_optimizer.cc:47-197) for P independent problems.  loop_detector::select_loop_candidate_via_Sim3
+ * (module/loop_detector.cc:388-397) runs it once per loop candidate that passed the Sim3 RANSAC, with chi_sq 10 and
+ * num_iter 10; all such candidates (or the candidates of many query keyframes) go in one call.
+ * Problem p owns the valid matches [match_offsets[p], match_offsets[p+1]) -- those of :91-126 in idx1 order, one per
+ * mutual edge pair: pos_w_1 / pos_w_2 (N x 3) the positions of keyframe 1's and keyframe 2's landmark, obs_1 / obs_2
+ * (N x 2) the float undist_keypts_ of idx1 in keyframe 1 and idx2 in keyframe 2, inv_sigma_sq_1 / _2 (N) the keyframes'
+ * inv_level_sigma_sq_ at those keypoints' octaves.  rot_1w / trans_1w and rot_2w / trans_2w (P x 9 row-major, P x 3): the
+ * keyframes' poses; rot_12_in / trans_12_in / scale_12_in: the caller's Sim3_12, built as g2o::Sim3(R, t, s) (the RANSAC's
+ * float scale widened to double, as that constructor does).  cams[p]: the camera of both keyframes; the edges read fx,
+ * fy, cx, cy only (the perspective and fisheye models share the perspective edge; equirectangular keyframes are not
+ * supported).  fix_scale: the reference's setup_type != Monocular (system.cc:140).
+ * Per problem: optimize(5) over every match; a match is an outlier when either edge fails chi2 < chi_sq; when fewer than
+ * 10 matches survive, num_inliers 0 and rot_12 / trans_12 / scale_12 are the input bits (the reference returns before it
+ * writes the Sim3), with the outlier flags already written.  Otherwise optimize(num_iter) over the survivors, the matches
+ * with chi_sq < chi2 of either edge become outliers too, num_inliers counts the rest, and rot_12 (row-major, the estimate's
+ * toRotationMatrix()), trans_12 and scale_12 are the optimised Sim3.  inlier_out[i] (N) is 0 where the reference sets the
+ * match to nullptr, 1 elsewhere.  A problem with no matches gets num_inliers 0 and its input Sim3.
+ * Every output of every problem is written.  There is no per-problem size limit; num_iter above 1000 returns
+ * PLP_ERR_CAPACITY before anything is launched or written.  PLP_ERR_INVALID, nothing launched and nothing written: a null
+ * pointer, offsets not non-decreasing from 0, a negative size, or a chi_sq that is not finite and positive.  Host arrays
+ * in and out; returns when the results are written.  g2o's Sim3, its Levenberg driver and its numeric Jacobian are
+ * restated in csrc/sim3optmath.h (parity with g2o unpinned); the device's sin / cos / exp are not glibc's, so results
+ * agree with the CPU oracle to a tolerance, not bit for bit. */
+PLP_API plp_status plp_sim3_optimize(plp_ctx *ctx, int num_problems, const int32_t *match_offsets /* P + 1 */,
+                                     const plp_camera *cams /* P: fx, fy, cx, cy read */,
+                                     const double *rot_1w /* P x 9 */, const double *trans_1w /* P x 3 */,
+                                     const double *rot_2w /* P x 9 */, const double *trans_2w /* P x 3 */,
+                                     const double *rot_12_in /* P x 9 */, const double *trans_12_in /* P x 3 */,
+                                     const double *scale_12_in /* P */, const double *pos_w_1 /* N x 3 */,
+                                     const double *pos_w_2 /* N x 3 */, const float *obs_1 /* N x 2 */,
+                                     const float *obs_2 /* N x 2 */, const float *inv_sigma_sq_1 /* N */,
+                                     const float *inv_sigma_sq_2 /* N */, float chi_sq, int num_iter, int fix_scale,
+                                     int32_t *num_inliers_out /* P */, double *rot_12_out /* P x 9 */,
+                                     double *trans_12_out /* P x 3 */, double *scale_12_out /* P */,
+                                     uint8_t *inlier_out /* N */);
+
+/* ------------------------------------------------------------------------ */
 /* plane RANSAC  (planar_mapping_module.{h,cc})                              */
 /* ------------------------------------------------------------------------ */
 /* Planar_Mapping_module::estimate_plane_sequential_RANSAC (planar_mapping_module.cc:412-591, mode 0) and

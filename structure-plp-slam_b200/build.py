@@ -42,6 +42,7 @@ FILE_FLAGS = {
     "bow_db.cu": NO_FMA,
     "pnp.cu": NO_FMA,
     "sim3.cu": NO_FMA,
+    "sim3_opt.cu": NO_FMA,
 }
 
 

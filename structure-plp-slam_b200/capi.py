@@ -545,6 +545,34 @@ class Context:
             scale.ctypes.data_as(_P)))
         return valid[:P].copy(), num[:P].copy(), rot[:P].reshape(P, 3, 3).copy(), trans[:P].copy(), scale[:P].copy()
 
+    # ------------------------------------------------------------------ optimize::transform_optimizer
+    def sim3_optimize(self, match_offsets, cams, rot_1w, trans_1w, rot_2w, trans_2w, rot_12, trans_12, scale_12, pos_w_1,
+                      pos_w_2, obs_1, obs_2, inv_sigma_sq_1, inv_sigma_sq_2, chi_sq=10.0, num_iter=10, fix_scale=False):
+        """transform_optimizer::optimize of P problems in one call (plp_sim3_optimize).  match_offsets: P + 1; cams: P
+        Camera structs (fx, fy, cx, cy read); rot_1w, rot_2w, rot_12: P x 3 x 3; trans_1w, trans_2w, trans_12: P x 3;
+        scale_12: P (double); pos_w_1, pos_w_2: N x 3; obs_1, obs_2: N x 2 float; inv_sigma_sq_1, _2: N float.  Returns
+        (num_inliers (P), rot_12 (P x 3 x 3), trans_12 (P x 3), scale_12 (P), inlier (N, uint8))."""
+        off = np.ascontiguousarray(match_offsets, np.int32)
+        P = len(off) - 1
+        if len(cams) != P:
+            raise PlpError(f"sim3_optimize: {len(cams)} cameras for {P} problems")
+        N = int(off[-1]) if P >= 0 and len(off) else 0
+        k = _Keep()
+        cam_arr = (Camera * max(P, 1))(*cams)
+        num = np.zeros(max(P, 1), np.int32)
+        rot = np.zeros((max(P, 1), 9))
+        trans = np.zeros((max(P, 1), 3))
+        scale = np.zeros(max(P, 1))
+        inl = np.zeros(max(N, 1), np.uint8)
+        d = lambda a: k.arr(np.reshape(a, -1), np.float64)
+        f = lambda a: k.arr(np.reshape(a, -1), np.float32)
+        self._check(self._lib.plp_sim3_optimize(
+            self._h, C.c_int(P), k.arr(off, np.int32), cam_arr, d(rot_1w), d(trans_1w), d(rot_2w), d(trans_2w), d(rot_12),
+            d(trans_12), d(scale_12), d(pos_w_1), d(pos_w_2), f(obs_1), f(obs_2), f(inv_sigma_sq_1), f(inv_sigma_sq_2),
+            C.c_float(chi_sq), C.c_int(num_iter), C.c_int(1 if fix_scale else 0), num.ctypes.data_as(_P),
+            rot.ctypes.data_as(_P), trans.ctypes.data_as(_P), scale.ctypes.data_as(_P), inl.ctypes.data_as(_P)))
+        return num[:P].copy(), rot[:P].reshape(P, 3, 3).copy(), trans[:P].copy(), scale[:P].copy(), inl[:N].copy()
+
     # ------------------------------------------------------------------ Planar_Mapping_module
     def plane_ransac(self, pos_w, valid, samples, cfg, eq0=(0, 0, 0, 0), err0=0.0):
         """estimate_plane_sequential_RANSAC (cfg['mode'] = 0) / update_plane_via_RANSAC (1) with caller-drawn index samples

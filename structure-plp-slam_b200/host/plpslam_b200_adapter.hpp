@@ -24,6 +24,7 @@
 #include <set>
 #include <stdexcept>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include <opencv2/core.hpp>
@@ -593,6 +594,119 @@ inline std::vector<sim3_candidate_result> sim3_ransac_candidates(PLPSLAM::data::
             out[k].trans_12(r) = trans[3 * k + r];
         }
         out[k].scale_12 = scale[k];
+    }
+    return out;
+}
+
+// camera::base::model_type_ == Equirectangular (camera/base.h); a camera type without that member has no such model
+template <class Camera>
+inline auto is_equirectangular(const Camera *c, int) -> decltype((void)c->model_type_, bool()) {
+    return c->model_type_ == std::remove_cv_t<decltype(c->model_type_)>::Equirectangular;
+}
+template <class Camera>
+inline bool is_equirectangular(const Camera *, long) { return false; }
+
+// ---- loop_detector::select_loop_candidate_via_Sim3's Sim3 optimisation (module/loop_detector.cc:394-397) for every
+// candidate in one call ----
+// run[i]: candidate i reached the optimiser (not will_be_erased(), >= 20 BoW matches, a valid RANSAC Sim3) and
+// match_keyframes_mutually has filled matched_lms[i].  sim3s[i] is the candidate's g2o::Sim3(rot_12, trans_12, scale_12)
+// built from the RANSAC result (scale widened from float); on return it is the optimised Sim3 -- or unchanged where the
+// reference returns 0 before writing it.  Each candidate's matches are transform_optimizer::optimize's
+// (optimize/transform_optimizer.cc:91-126): idx1 in order, skipping null and will_be_erased() landmarks and landmarks
+// that keyframe 2 does not observe (get_index_in_keyframe as a lookup in get_observations()), with both keyframes'
+// undist_keypts_ and inv_level_sigma_sq_.  Outliers are set to nullptr in matched_lms[i], as the reference does.
+// cam: the camera of both keyframes (camera_of() for a perspective camera, the fisheye camera's own fx_ .. cy_);
+// fix_scale: fix_scale_in_Sim3_estimation_.  Returns num_optimized_inliers per candidate (0 where run[i] is false).
+// Throws on size mismatches, on keyframes with different cameras, and on equirectangular keyframes (not supported).
+struct sim3_estimate {
+    PLPSLAM::Mat33_t rot_12;
+    PLPSLAM::Vec3_t trans_12;
+    double scale_12 = 1.0;
+};
+
+inline std::vector<unsigned> sim3_optimize_candidates(PLPSLAM::data::keyframe *cur_keyfrm,
+                                                      const std::vector<PLPSLAM::data::keyframe *> &candidates,
+                                                      std::vector<std::vector<PLPSLAM::data::landmark *>> &matched_lms,
+                                                      std::vector<sim3_estimate> &sim3s, const std::vector<bool> &run,
+                                                      bool fix_scale, const plp_camera &cam, float chi_sq = 10,
+                                                      unsigned num_iter = 10) {
+    const size_t K = candidates.size();
+    if (matched_lms.size() != K || sim3s.size() != K || run.size() != K)
+        throw std::invalid_argument("plpslam_b200::sim3_optimize_candidates: candidates, matched_lms, sim3s and run differ in size");
+    if (is_equirectangular(cur_keyfrm->camera_, 0))
+        throw std::invalid_argument("plpslam_b200::sim3_optimize_candidates: equirectangular keyframes are not supported");
+    const auto keyfrm_1_lms = cur_keyfrm->get_landmarks();
+    const PLPSLAM::Mat33_t rot_1w = cur_keyfrm->get_rotation();
+    const PLPSLAM::Vec3_t trans_1w = cur_keyfrm->get_translation();
+    std::vector<size_t> cand;  // problem -> candidate
+    std::vector<std::vector<unsigned>> idx1s;  // problem -> idx1 of each valid match
+    std::vector<int32_t> off(1, 0);
+    std::vector<plp_camera> cams;
+    std::vector<double> r1, t1, r2, t2, r12, t12, s12, pos_1, pos_2;
+    std::vector<float> obs_1, obs_2, w_1, w_2;
+    for (size_t k = 0; k < K; ++k) {
+        if (!run[k]) continue;
+        auto *keyfrm_2 = candidates[k];
+        if (keyfrm_2->camera_ != cur_keyfrm->camera_)
+            throw std::invalid_argument("plpslam_b200::sim3_optimize_candidates: the keyframes' cameras differ");
+        const PLPSLAM::Mat33_t rot_2w = keyfrm_2->get_rotation();
+        const PLPSLAM::Vec3_t trans_2w = keyfrm_2->get_translation();
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) {
+                r1.push_back(rot_1w(r, c));
+                r2.push_back(rot_2w(r, c));
+                r12.push_back(sim3s[k].rot_12(r, c));
+            }
+            t1.push_back(trans_1w(r));
+            t2.push_back(trans_2w(r));
+            t12.push_back(sim3s[k].trans_12(r));
+        }
+        s12.push_back(sim3s[k].scale_12);
+        cams.push_back(cam);
+        std::vector<unsigned> idx;
+        for (unsigned idx1 = 0; idx1 < matched_lms[k].size(); ++idx1) {  // :91-126
+            auto *lm_2 = matched_lms[k][idx1];
+            if (!lm_2) continue;
+            auto *lm_1 = keyfrm_1_lms.at(idx1);
+            if (!lm_1 || !lm_2) continue;
+            if (lm_1->will_be_erased() || lm_2->will_be_erased()) continue;
+            // get_index_in_keyframe(keyfrm_2) (data/landmark.cc:156-167): the observation index, or -1
+            const auto obs = lm_2->get_observations();
+            const auto found = obs.find(keyfrm_2);
+            if (found == obs.end()) continue;
+            const auto &kp_1 = cur_keyfrm->undist_keypts_.at(idx1);
+            const auto &kp_2 = keyfrm_2->undist_keypts_.at(found->second);
+            const PLPSLAM::Vec3_t p1 = lm_1->get_pos_in_world(), p2 = lm_2->get_pos_in_world();
+            for (int c = 0; c < 3; ++c) pos_1.push_back(p1(c)), pos_2.push_back(p2(c));
+            obs_1.push_back(kp_1.pt.x), obs_1.push_back(kp_1.pt.y);
+            obs_2.push_back(kp_2.pt.x), obs_2.push_back(kp_2.pt.y);
+            w_1.push_back(cur_keyfrm->inv_level_sigma_sq_.at(kp_1.octave));
+            w_2.push_back(keyfrm_2->inv_level_sigma_sq_.at(kp_2.octave));
+            idx.push_back(idx1);
+        }
+        off.push_back(off.back() + (int32_t)idx.size());
+        cand.push_back(k);
+        idx1s.push_back(std::move(idx));
+    }
+    const size_t P = cand.size(), N = (size_t)off.back();
+    std::vector<int32_t> num_inliers(P + 1);
+    std::vector<double> rot(P * 9 + 1), trans(P * 3 + 1), scale(P + 1);
+    std::vector<uint8_t> inlier(N + 1);
+    check(plp_sim3_optimize(thread_ctx(), (int)P, off.data(), cams.data(), r1.data(), t1.data(), r2.data(), t2.data(),
+                            r12.data(), t12.data(), s12.data(), pos_1.data(), pos_2.data(), obs_1.data(), obs_2.data(),
+                            w_1.data(), w_2.data(), chi_sq, (int)num_iter, fix_scale ? 1 : 0, num_inliers.data(), rot.data(),
+                            trans.data(), scale.data(), inlier.data()));
+    std::vector<unsigned> out(K, 0);
+    for (size_t p = 0; p < P; ++p) {
+        const size_t k = cand[p];
+        for (size_t i = 0; i < idx1s[p].size(); ++i)
+            if (!inlier[off[p] + i]) matched_lms[k][idx1s[p][i]] = nullptr;
+        for (int r = 0; r < 3; ++r) {
+            for (int c = 0; c < 3; ++c) sim3s[k].rot_12(r, c) = rot[9 * p + 3 * r + c];
+            sim3s[k].trans_12(r) = trans[3 * p + r];
+        }
+        sim3s[k].scale_12 = scale[p];
+        out[k] = (unsigned)num_inliers[p];
     }
     return out;
 }
