@@ -16,7 +16,7 @@
 //              restatement against cv2 (std::sort seed order, libm cosf/sinf, sequential sums, swap-remove compaction).
 //   "det" mode {0, 0, 1}: the portable determinism rules the CUDA path implements bit-exactly: seeds ordered by gradient
 //              bin (descending) with raster order inside a bin (the bin lists of the original LSD and of OpenCV 3.4,
-//              the version the reference's README names), trigonometry by oracle/detmath.h, sums accumulated in 32
+//              the version the reference's README names), trigonometry by the library's detmath.h, sums accumulated in 32
 //              strided partials and combined by a fixed xor-tree, order-preserving compaction.
 #include "lines.h"
 

@@ -15,6 +15,7 @@
 #include <list>
 #include <vector>
 
+#define PLP_BRIEF_TABLE static const signed char
 #include "brief_pattern.inc"
 
 namespace {

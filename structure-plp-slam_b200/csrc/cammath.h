@@ -13,8 +13,8 @@
  * The products with the identity / K matrices are written out term by term in OpenCV's order (Matx: s = 0, s += a*b), so
  * even the sign of a zero matches.  tests/test_camera_oracle.py pins the oracle's copy to cv2 bit for bit.
  *
- * This file exists twice with identical text (oracle/cammath.h and structure-plp-slam_b200/csrc/cammath.h); the oracle
- * never includes product code and vice versa.  tests/test_camera_oracle.py checks that the copies stay identical.
+ * The library (nvcc -fmad=false), the oracle (g++ -ffp-contract=off) and the CPU emulators of tests/cta_emu compile
+ * this one text, so the device and the oracle evaluate the same expressions.
  */
 #ifndef PLP_CAMMATH_H
 #define PLP_CAMMATH_H

@@ -9,8 +9,8 @@
  * kernels: the classical minimax polynomials on [-pi/4, pi/4] (sin: degree 13, cos: degree 14) and the 4-interval
  * arctangent with an odd degree-23 polynomial.  Measured against glibc: max |err| < 2.3e-16 (tests/test_lines_oracle.py).
  *
- * This file exists twice with identical text (oracle/detmath.h and structure-plp-slam_b200/csrc/detmath.h); the oracle
- * never includes product code and vice versa.  tests/test_lines_oracle.py checks that the two copies stay identical.
+ * The library (nvcc -fmad=false), the oracle (g++ -ffp-contract=off) and the CPU emulators of tests/cta_emu compile
+ * this one text, so the device and the oracle evaluate the same expressions.
  */
 #ifndef PLP_DETMATH_H
 #define PLP_DETMATH_H

@@ -10,8 +10,8 @@
  * Both are the same mathematical objects as JacobiSVD's (up to the sign of v, which neither the inlier test nor the
  * score can see); they differ from Eigen's numbers by rounding only.  PARITY UNPINNED against Eigen (absent).
  *
- * This file exists twice with identical text (oracle/essmath.h and structure-plp-slam_b200/csrc/essmath.h); the oracle
- * never includes product code and vice versa.  tests/test_essential_oracle.py checks that the copies stay identical.
+ * The library (nvcc -fmad=false), the oracle (g++ -ffp-contract=off) and the CPU emulators of tests/cta_emu compile
+ * this one text, so the device and the oracle evaluate the same expressions.
  */
 #ifndef PLP_ESSMATH_H
 #define PLP_ESSMATH_H

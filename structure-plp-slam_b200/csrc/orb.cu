@@ -17,6 +17,8 @@
 #include "common.cuh"
 #include <cuda.h>  // CUtensorMap (types only: the encoder is fetched with cudaGetDriverEntryPoint, no libcuda link)
 #include <stdlib.h>
+// describe_kernel reads the pattern tables as uint2, so they are 16-byte aligned
+#define PLP_BRIEF_TABLE __device__ const signed char __align__(16)
 #include "brief_pattern.inc"
 #include "quadtree_kernels.cuh"
 

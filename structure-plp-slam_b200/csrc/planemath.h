@@ -7,7 +7,8 @@
  * header computes with the cyclic Jacobi kernel of essmath.h.  Sums run in index order.  The SIGN of the normal is
  * arbitrary in both formulations (distances and residuals do not see it).  PARITY UNPINNED against Eigen (absent).
  *
- * This file exists twice with identical text (oracle/planemath.h and structure-plp-slam_b200/csrc/planemath.h).
+ * The library (nvcc -fmad=false), the oracle (g++ -ffp-contract=off) and the CPU emulators of tests/cta_emu compile
+ * this one text.
  */
 #ifndef PLP_PLANEMATH_H
 #define PLP_PLANEMATH_H

@@ -31,8 +31,8 @@
  * ONE INTENDED DEVIATION: when qr_solve meets a zero column (eta == 0, :786-790) the reference returns without writing X,
  * so gauss_newton adds an uninitialised (or the previous iteration's) step; here X = 0.
  *
- * This file exists twice with identical text (oracle/pnpmath.h and structure-plp-slam_b200/csrc/pnpmath.h); the oracle
- * never includes product code and vice versa.  tests/test_pnp_oracle.py checks that the copies stay identical.
+ * The library (nvcc -fmad=false), the oracle (g++ -ffp-contract=off) and the CPU emulators of tests/cta_emu compile
+ * this one text, so the device and the oracle evaluate the same expressions.
  */
 #ifndef PLP_PNPMATH_H
 #define PLP_PNPMATH_H

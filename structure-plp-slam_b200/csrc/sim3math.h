@@ -27,8 +27,8 @@
  *      Ties need degenerate samples (coincident or collinear points).
  * With NaN in N no eigenvalue passes the scan and the reference reads column -1; here column 0 (NaN input only).
  *
- * This file exists twice with identical text (oracle/sim3math.h and structure-plp-slam_b200/csrc/sim3math.h); the oracle
- * never includes product code and vice versa.  tests/test_sim3_oracle.py checks that the copies stay identical.
+ * The library (nvcc -fmad=false), the oracle (g++ -ffp-contract=off) and the CPU emulators of tests/cta_emu compile
+ * this one text, so the device and the oracle evaluate the same expressions.
  */
 #ifndef PLP_SIM3MATH_H
 #define PLP_SIM3MATH_H

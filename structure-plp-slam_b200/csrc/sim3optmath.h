@@ -32,9 +32,9 @@
  * already restates (se3.cuh R_to_quat / quat_to_R on the device, g2o_lite.hpp quat_from_matrix / quat_to_matrix in the
  * oracle; the same arithmetic), reached through s3o_R_to_quat / s3o_quat_to_R below.
  *
- * This file exists twice with identical text (oracle/sim3optmath.h and structure-plp-slam_b200/csrc/sim3optmath.h); the
- * oracle defines SIM3OPT_WITH_G2O_LITE before including it and never includes product code, and vice versa.
- * tests/test_sim3_opt_oracle.py checks that the copies stay identical.
+ * The library (nvcc -fmad=false), the oracle (g++ -ffp-contract=off) and the CPU emulators of tests/cta_emu compile
+ * this one text, so the device and the oracle evaluate the same expressions.  The oracle defines SIM3OPT_WITH_G2O_LITE
+ * before including it and takes the quaternion conversions from its g2o_lite.hpp.
  */
 #ifndef PLP_SIM3OPTMATH_H
 #define PLP_SIM3OPTMATH_H

@@ -185,16 +185,13 @@ def crafted():
 
 
 # ---------------------------------------------------------------------------------------------------- native oracle
-def build_oracle(out_dir):
-    """Compiles tests/bow_db_oracle.cc into out_dir; returns the ctypes library."""
+def oracle():
+    """The oracle library with the restypes of oracle/bow_db_oracle.cc's entries declared."""
     import ctypes
-    import subprocess
 
-    so = Path(out_dir) / "libbow_db_oracle.so"
-    src = Path(__file__).resolve().parent / "bow_db_oracle.cc"
-    subprocess.run(["g++", "-O3", "-std=c++17", "-ffp-contract=off", "-fno-fast-math", "-shared", "-fPIC", str(src),
-                    "-o", str(so)], check=True)
-    lib = ctypes.CDLL(str(so))
+    import oracle_api
+
+    lib = oracle_api.lib()
     lib.orc_bow_db_create.restype = ctypes.c_void_p
     lib.orc_bow_score.restype = ctypes.c_float
     for f in ("orc_bow_db_destroy", "orc_bow_db_add", "orc_bow_db_erase", "orc_bow_db_reloc", "orc_bow_db_loop"):
@@ -220,7 +217,7 @@ def _graph_csr(cov):
 
 
 class NativeDatabase:
-    """The C++ restatement (tests/bow_db_oracle.cc) behind the same methods as Database."""
+    """The C++ restatement (oracle/bow_db_oracle.cc) behind the same methods as Database."""
 
     def __init__(self, lib):
         import ctypes

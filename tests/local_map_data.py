@@ -2,12 +2,10 @@
 monocular points): local maps derived from earlier keyframes of scene.PlanarSequence, distractor rows for every
 can_observe gate, and the oracle chain motion_based_track -> search_local_landmarks -> pose_optimize -> outlier drop.
 
-The can_observe restatement is tests/local_map_oracle.cc (built next to the oracle library); the matcher and the pose
-optimiser are the oracle library's."""
+The can_observe restatement (oracle/local_map_oracle.cc), the matcher and the pose optimiser are the oracle library's."""
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 from pathlib import Path
 
 import numpy as np
@@ -16,7 +14,6 @@ import oracle_api
 import synth
 
 ROOT = Path(__file__).resolve().parent.parent
-ORACLE_LIB = ROOT / "oracle" / "_build" / "liblocal_map_oracle.so"
 _P = C.c_void_p
 NUM_LEVELS = 8
 MARGIN = 5.0        # tracking_module.cc:976-981 (20 right after a relocalisation)
@@ -33,21 +30,6 @@ def logf(x) -> np.float32:
 LOG_SF = logf(1.2)  # frame::log_scale_factor_ = std::log(scale_factor_) on floats
 SF = synth.scale_factors()
 ISIG = synth.inv_level_sigma_sq()
-
-_LIB = None
-
-
-def oracle_lib():
-    global _LIB
-    if _LIB is None:
-        if not ORACLE_LIB.exists():  # normally built by __graft_entry__.build()
-            ORACLE_LIB.parent.mkdir(exist_ok=True)
-            res = subprocess.run(["g++", "-O3", "-std=c++17", "-fPIC", "-ffp-contract=off", "-fno-fast-math", "-shared",
-                                  str(ROOT / "tests" / "local_map_oracle.cc"), "-o", str(ORACLE_LIB)],
-                                 capture_output=True, text=True)
-            assert res.returncode == 0, res.stderr
-        _LIB = C.CDLL(str(ORACLE_LIB))
-    return _LIB
 
 
 def cam_center(T):
@@ -75,10 +57,10 @@ def can_observe(cam, T, lms, skip=None):
     obs = np.zeros(max(m, 1), np.uint8)
     rx, ry = np.zeros(max(m, 1), np.float32), np.zeros(max(m, 1), np.float32)
     lvl, gate = np.zeros(max(m, 1), np.int32), np.zeros(max(m, 1), np.int32)
-    oracle_lib().lmo_can_observe(C.byref(ocam), T.ctypes.data_as(_P), C.c_int(m), *[a.ctypes.data_as(_P) for a in arrs],
-                                 sk.ctypes.data_as(_P), C.c_float(LOG_SF), C.c_int(NUM_LEVELS), obs.ctypes.data_as(_P),
-                                 rx.ctypes.data_as(_P), ry.ctypes.data_as(_P), lvl.ctypes.data_as(_P),
-                                 gate.ctypes.data_as(_P))
+    oracle_api.lib().lmo_can_observe(C.byref(ocam), T.ctypes.data_as(_P), C.c_int(m),
+                                     *[a.ctypes.data_as(_P) for a in arrs], sk.ctypes.data_as(_P), C.c_float(LOG_SF),
+                                     C.c_int(NUM_LEVELS), obs.ctypes.data_as(_P), rx.ctypes.data_as(_P),
+                                     ry.ctypes.data_as(_P), lvl.ctypes.data_as(_P), gate.ctypes.data_as(_P))
     return obs[:m], rx[:m], ry[:m], lvl[:m], gate[:m]
 
 

@@ -3,19 +3,18 @@ module::local_map_updater, local_map_updater.cc), restated in Python, and the ma
 
 The restatement walks the voted keyframes in ascending table index: the reference walks them in the iteration order of
 an unordered_map keyed by pointer, which the device replaces by that canonical order (DESIGN.md §3.17).  The C++
-restatement in tests/local_map_update_oracle.cc must give the same lists; the tests check both against each other and
+restatement in oracle/local_map_update_oracle.cc must give the same lists; the tests check both against each other and
 against the device code."""
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
 
 import numpy as np
 
 import local_map_data as lmd
+import oracle_api
 
 ROOT = lmd.ROOT
-ORACLE_LIB = ROOT / "oracle" / "_build" / "liblocal_map_update_oracle.so"
 MAX_NUM_LOCAL_KEYFRMS = 60   # tracking_module.cc:873
 WEIGHT_THR = 15              # graph_node::weight_thr_ (graph_node.h)
 TOP_N_COV = 10               # local_map_updater.cc:179
@@ -110,28 +109,12 @@ def local_rows(snap, local_lm):
 
 
 # ---- the C++ restatement ---------------------------------------------------------------------------------------------
-_LIB = None
-
-
-def oracle_lib():
-    global _LIB
-    if _LIB is None:
-        if not ORACLE_LIB.exists():  # normally built by __graft_entry__.build()
-            ORACLE_LIB.parent.mkdir(exist_ok=True)
-            res = subprocess.run(["g++", "-O2", "-std=c++17", "-fPIC", "-shared",
-                                  str(ROOT / "tests" / "local_map_update_oracle.cc"), "-o", str(ORACLE_LIB)],
-                                 capture_output=True, text=True)
-            assert res.returncode == 0, res.stderr
-        _LIB = C.CDLL(str(ORACLE_LIB))
-    return _LIB
-
-
 def _i32(a):
     return np.ascontiguousarray(a, np.int32)
 
 
 def oracle_update(snap, tracked_lm):
-    """tests/local_map_update_oracle.cc on one frame; the same result as update_local_map (None: no keyframe voted)."""
+    """oracle/local_map_update_oracle.cc on one frame; the same result as update_local_map (None: no keyframe voted)."""
     K, L = len(snap["kf_erased"]), len(snap["lm_erased"])
     arrs = [_i32(tracked_lm), np.ascontiguousarray(snap["lm_erased"], np.uint8), _i32(snap["obs_offsets"]),
             _i32(snap["obs_kf"]), np.ascontiguousarray(snap["kf_erased"], np.uint8), _i32(snap["row_offsets"]),
@@ -140,9 +123,9 @@ def oracle_update(snap, tracked_lm):
     out_kf = np.zeros(max(K, 1), np.int32)
     out_lm = np.zeros(max(L, 1), np.int32)
     n = np.zeros(4, np.int32)  # num_local_kf, num_local_lm, nearest, num_voted
-    ok = oracle_lib().lmuo_update_local_map(C.c_int(len(tracked_lm)), C.c_int(K), C.c_int(L),
-                                            *[a.ctypes.data_as(_P) for a in arrs], out_kf.ctypes.data_as(_P),
-                                            out_lm.ctypes.data_as(_P), n.ctypes.data_as(_P))
+    ok = oracle_api.lib().lmuo_update_local_map(C.c_int(len(tracked_lm)), C.c_int(K), C.c_int(L),
+                                                *[a.ctypes.data_as(_P) for a in arrs], out_kf.ctypes.data_as(_P),
+                                                out_lm.ctypes.data_as(_P), n.ctypes.data_as(_P))
     if not ok:
         return None
     return dict(local_kf=[int(x) for x in out_kf[:n[0]]], nearest=int(n[2]), local_lm=[int(x) for x in out_lm[:n[1]]],
@@ -295,7 +278,7 @@ def bench_setup(pkg, ctx, batch=512, seed=1234, track_ctx=None):
 
 
 def oracle_update_batch(snap, n_kp, matched, num_valid, last_offsets, max_local):
-    """tests/local_map_update_oracle.cc's lmuo_update_batch: the native host walk of a motion-tracked batch (matched:
+    """oracle/local_map_update_oracle.cc's lmuo_update_batch: the native host walk of a motion-tracked batch (matched:
     batch x cap last-frame rows).  -> (offsets, local landmarks per row of the concatenated lists, last_local_idx)."""
     B, cap = matched.shape
     K, L = len(snap["kf_erased"]), len(snap["lm_erased"])
@@ -307,7 +290,7 @@ def oracle_update_batch(snap, n_kp, matched, num_valid, last_offsets, max_local)
             np.ascontiguousarray(snap["kf_erased"], np.uint8), _i32(snap["row_offsets"]), _i32(snap["row_lm"]),
             _i32(snap["cov_offsets"]), _i32(snap["cov_kf"]), _i32(snap["child_offsets"]), _i32(snap["child_kf"]),
             _i32(snap["parent"]), offs, out_lm, lli]
-    oracle_lib().lmuo_update_batch(C.c_int(B), C.c_int(cap), C.c_int(K), C.c_int(L), C.c_int(max_local),
-                                   *[a.ctypes.data_as(_P) for a in arrs])
+    oracle_api.lib().lmuo_update_batch(C.c_int(B), C.c_int(cap), C.c_int(K), C.c_int(L), C.c_int(max_local),
+                                       *[a.ctypes.data_as(_P) for a in arrs])
     lm = np.concatenate([out_lm[b * max_local:b * max_local + offs[b + 1] - offs[b]] for b in range(B)])
     return offs, lm, lli[:int(last_offsets[B])]

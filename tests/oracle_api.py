@@ -24,15 +24,19 @@ class OCamera(C.Structure):
                 ("setup_type", C.c_int32)]
 
 
-def build_oracle():
-    srcs = list(ORACLE_DIR.glob("*.cc")) + list(ORACLE_DIR.glob("*.h")) + list(ORACLE_DIR.glob("*.inc"))
-    so = ORACLE_DIR / "liboracle.so"
-    if so.exists() and all(so.stat().st_mtime >= s.stat().st_mtime for s in srcs):
-        return so
-    res = subprocess.run(["make", "-C", str(ORACLE_DIR), "-j8"], capture_output=True, text=True)
-    if res.returncode != 0:
-        raise RuntimeError("oracle build failed:\n" + res.stdout + res.stderr)
-    return so
+_LIB = None
+
+
+def lib():
+    """liboracle.so, loaded once per process.  oracle/Makefile tracks every header the library includes, so running make
+    first only rebuilds what changed (and writes nothing when it is up to date)."""
+    global _LIB
+    if _LIB is None:
+        res = subprocess.run(["make", "-C", str(ORACLE_DIR), "-j8"], capture_output=True, text=True)
+        if res.returncode != 0:
+            raise RuntimeError("oracle build failed:\n" + res.stdout + res.stderr)
+        _LIB = C.CDLL(str(ORACLE_DIR / "liboracle.so"))
+    return _LIB
 
 
 def _a(x, dt):
@@ -53,7 +57,7 @@ def as_camera(c) -> OCamera:
 
 class Oracle:
     def __init__(self):
-        self.lib = C.CDLL(str(build_oracle()))
+        self.lib = lib()
         L = self.lib
         for f in ("orc_hamming_32", "orc_hamming_64", "orc_match_frame_and_landmarks",
                   "orc_match_current_and_last_frames", "orc_match_frame_and_landmarks_line",

@@ -1,16 +1,13 @@
 """Stereo rectification test data: the StereoRectifier configs the reference ships plus synthetic ones, the CPU oracle of
-rectification (tests/rectify_oracle.cc, which __graft_entry__.build() compiles next to the oracle library) and its
-cv2 counterparts."""
+rectification (oracle/rectify_oracle.cc, part of the oracle library) and its cv2 counterparts."""
 from __future__ import annotations
 
 import ctypes as C
-import subprocess
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-CSRC = ROOT / "structure-plp-slam_b200" / "csrc"
+import oracle_api
+
 _P = C.c_void_p
 
 PERSPECTIVE, FISHEYE = 0, 1
@@ -108,41 +105,15 @@ def k_rect32(rect):
 
 
 # ---- the oracle
-ORACLE_LIB = ROOT / "oracle" / "_build" / "librectify_oracle.so"   # built by __graft_entry__.build()
-
-
-def build_emu(out_dir: Path):
-    """tests/cta_emu/rectify_emu.cc: the kernel header compiled for the CPU."""
-    so = out_dir / "librectify_emu.so"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-fno-fast-math",
-           f"-I{CSRC}", f"-I{ROOT / 'tests' / 'cta_emu'}", str(ROOT / "tests" / "cta_emu" / "rectify_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
-
-
-_ORACLE = None
-
-
-def oracle():
-    """The rectification oracle library (tests/rectify_oracle.cc)."""
-    global _ORACLE
-    if _ORACLE is None:
-        if not ORACLE_LIB.exists():
-            raise RuntimeError(f"{ORACLE_LIB} is missing: run __graft_entry__.build()")
-        _ORACLE = C.CDLL(str(ORACLE_LIB))
-    return _ORACLE
-
-
 def oracle_maps_raw(model, K, D, R, rect, rows, cols):
     """-> (status, map_x, map_y)."""
     mx = np.zeros((rows, cols), np.float32) if rows > 0 and cols > 0 else np.zeros(1, np.float32)
     my = np.zeros_like(mx)
     Kd, Dd, Rd = (np.ascontiguousarray(a, np.float64).ravel() for a in (K, d5(D), R))
     Kr = np.ascontiguousarray(rect, np.float64)
-    st = oracle().orc_rect_maps(C.c_int(model), Kd.ctypes.data_as(_P), Dd.ctypes.data_as(_P), Rd.ctypes.data_as(_P),
-                                Kr.ctypes.data_as(_P), C.c_int(rows), C.c_int(cols), mx.ctypes.data_as(_P),
-                                my.ctypes.data_as(_P))
+    st = oracle_api.lib().orc_rect_maps(C.c_int(model), Kd.ctypes.data_as(_P), Dd.ctypes.data_as(_P),
+                                        Rd.ctypes.data_as(_P), Kr.ctypes.data_as(_P), C.c_int(rows), C.c_int(cols),
+                                        mx.ctypes.data_as(_P), my.ctypes.data_as(_P))
     return st, mx, my
 
 
@@ -164,9 +135,10 @@ def oracle_remap(src, map_x, map_y, out=None):
     if out is None:
         out = np.zeros((orows, ocols), np.uint8)
     assert out.strides[1] == 1
-    oracle().orc_remap_linear_u8(src.ctypes.data_as(_P), C.c_int(src.shape[0]), C.c_int(src.shape[1]),
-                                 C.c_size_t(src.strides[0]), map_x.ctypes.data_as(_P), map_y.ctypes.data_as(_P),
-                                 C.c_int(orows), C.c_int(ocols), out.ctypes.data_as(_P), C.c_size_t(out.strides[0]))
+    oracle_api.lib().orc_remap_linear_u8(src.ctypes.data_as(_P), C.c_int(src.shape[0]), C.c_int(src.shape[1]),
+                                         C.c_size_t(src.strides[0]), map_x.ctypes.data_as(_P), map_y.ctypes.data_as(_P),
+                                         C.c_int(orows), C.c_int(ocols), out.ctypes.data_as(_P),
+                                         C.c_size_t(out.strides[0]))
     return out
 
 

@@ -3,30 +3,20 @@ common-word counts, scores and the candidate selection, each equal to the Python
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import bow_db_data as bdd
+import emu_build
 
-ROOT = Path(__file__).resolve().parents[1]
 _P = C.c_void_p
 NUM_WORDS = 5000
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libbowdb_emu.so"
-    csrc = ROOT / "structure-plp-slam_b200" / "csrc"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", f"-I{csrc}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "bowdb_emu.cc"), "-o", str(so)]
-    subprocess.run(cmd, check=True)
-    return C.CDLL(str(so))
+    return emu_build.emu("bowdb_emu", tmp_path_factory)
 
 
 def _ptr(a):

@@ -1,5 +1,5 @@
 """The keyframe BoW database on the GPU (plp_bow_db) against the Python restatement of data::bow_database
-(tests/bow_db_data.py) and its C++ restatement (tests/bow_db_oracle.cc): candidate lists equal, scores bit-equal, at 1,
+(tests/bow_db_data.py) and its C++ restatement (oracle/bow_db_oracle.cc): candidate lists equal, scores bit-equal, at 1,
 10, 128 and 3000 keyframes, single-keyframe adds and erases on a populated database, and the refusals."""
 from __future__ import annotations
 
@@ -32,8 +32,8 @@ def load(plp, ctx, vocab, db, K, W):
 
 
 @pytest.fixture(scope="module")
-def orc(tmp_path_factory):
-    return bdd.build_oracle(tmp_path_factory.mktemp("bow_db_oracle"))
+def orc():
+    return bdd.oracle()
 
 
 def check(dev, db, K, queries, loops, cov, orc=None):

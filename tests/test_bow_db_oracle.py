@@ -1,9 +1,7 @@
-"""The C++ restatement of data::bow_database (tests/bow_db_oracle.cc, the reference's containers) against the independent
+"""The C++ restatement of data::bow_database (oracle/bow_db_oracle.cc, the reference's containers) against the independent
 Python restatement (tests/bow_db_data.py): candidate list for list and score for score, on the boundary scene, seeded
 synthetic databases and vectors over the shipped vocabulary's golden subtree."""
 from __future__ import annotations
-
-import shutil
 
 import numpy as np
 import pytest
@@ -12,10 +10,8 @@ import bow_db_data as bdd
 
 
 @pytest.fixture(scope="module")
-def lib(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    return bdd.build_oracle(tmp_path_factory.mktemp("bow_db_oracle"))
+def lib():
+    return bdd.oracle()
 
 
 def _same(lib, db, queries, loops, cov):

@@ -2,16 +2,13 @@
 tests/cta_emu (see test_cta_emu.py): batch x capacity slots, per-frame counts (one frame empty), untouched slots past a
 frame's count, and the undistorted keypoints and bearings equal to the oracle bit for bit."""
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
 import camera_data as cd
+import emu_build
 
-ROOT = Path(__file__).resolve().parent.parent
 _P = C.c_void_p
 KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4"), ("response", "<f4"),
                      ("octave", "<i4"), ("class_id", "<i4")])
@@ -19,15 +16,7 @@ KP_DTYPE = np.dtype([("x", "<f4"), ("y", "<f4"), ("size", "<f4"), ("angle", "<f4
 
 @pytest.fixture(scope="module")
 def cam_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libcamera_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "camera_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("camera_emu", tmp_path_factory, opt="-O1")
 
 
 @pytest.mark.parametrize("name", list(cd.ALL))

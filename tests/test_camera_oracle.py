@@ -7,7 +7,6 @@ on icdist < 0).  For points where that iteration oscillates without converging -
 synthetic strong barrel distortion -- cv2 4.13 returns other values (for the shipped EuRoC model it returns the exact
 inverse of the distortion).  Those points are listed here, not compared; they never arise inside the image of a shipped
 configuration, which the tests below check point by point."""
-from pathlib import Path
 
 import numpy as np
 import pytest
@@ -15,7 +14,6 @@ import pytest
 import camera_data as cd
 import synth
 
-ROOT = Path(__file__).resolve().parent.parent
 cv2 = pytest.importorskip("cv2")
 
 
@@ -45,10 +43,6 @@ def _reprojects(model, K, D, x, y, ux, uy, tol=1e-3):
         xd = X * c + 2 * k[2] * X * Y + k[3] * (r2 + 2 * X * X)
         yd = Y * c + k[2] * (r2 + 2 * Y * Y) + 2 * k[3] * X * Y
     return (np.abs(xd * fx + cx - x) < tol) & (np.abs(yd * fy + cy - y) < tol)
-
-
-def test_cammath_copies_identical():
-    assert (ROOT / "oracle" / "cammath.h").read_text() == (ROOT / "structure-plp-slam_b200" / "csrc" / "cammath.h").read_text()
 
 
 @pytest.mark.parametrize("name", list(cd.CONFIGS))

@@ -3,16 +3,13 @@ the same kernel text for the host (one host thread per CUDA thread, a pthread ba
 after the other) and this test compares it with the oracle bit for bit.  It checks the kernels' logic -- indexing, phase
 structure, replay bookkeeping -- in a container without a GPU; the GPU parity run is tests/test_plane_gpu.py."""
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+import emu_build
 import plane_data
 
-ROOT = Path(__file__).resolve().parent.parent
 _P = C.c_void_p
 
 
@@ -23,15 +20,7 @@ class Cfg(C.Structure):
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libplane_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "plane_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("plane_emu", tmp_path_factory, opt="-O1")
 
 
 def _run(emu, pts, valid, smp, cfg, eq0=(0, 0, 0, 0), err0=0.0):
@@ -79,15 +68,7 @@ def test_plane_kernels_on_cpu_failure_paths(emu, orc):
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def ess_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libess_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "essential_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("essential_emu", tmp_path_factory, opt="-O1")
 
 
 @pytest.mark.parametrize("seed", range(3))
@@ -115,15 +96,7 @@ def test_essential_kernels_on_cpu_match_oracle(ess_emu, orc, seed):
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def bow_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libbow_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "bow_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    lib = C.CDLL(str(so))
+    lib = emu_build.emu("bow_emu", tmp_path_factory, opt="-O1")
     lib.emu_bow_match.restype = C.c_uint
     return lib
 
@@ -214,15 +187,7 @@ def test_bow_match_kernel_on_cpu_matches_oracle(bow_emu, orc, seed):
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def fuse_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libfuse_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "fuse_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("fuse_emu", tmp_path_factory, opt="-O1")
 
 
 @pytest.mark.parametrize("seed,mode,stereo", [(0, 1, False), (1, 0, False), (2, 1, True)])
@@ -281,15 +246,7 @@ def test_fuse_points_kernel_on_cpu_matches_oracle(fuse_emu, orc, plp, seed, mode
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def pmatch_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libpmatch_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "pmatch_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("pmatch_emu", tmp_path_factory, opt="-O1")
 
 
 class _Grid(C.Structure):
@@ -375,15 +332,7 @@ def test_point_match_kernel_on_cpu_deferred_acceptance_path(pmatch_emu, orc, plp
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def poseopt_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libposeopt_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "poseopt_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("poseopt_emu", tmp_path_factory, opt="-O1")
 
 
 def _emu_pose_opt(emu, cam, scenes, with_lines):
@@ -491,15 +440,7 @@ def test_point_match_kernel_on_cpu_worklist_overflow(pmatch_emu, orc, plp):
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def lsdgrow_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "liblsdgrow_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "lsdgrow_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("lsdgrow_emu", tmp_path_factory, opt="-O1")
 
 
 def _lsd_grow_inputs(orc, img):
@@ -551,15 +492,7 @@ def test_lsd_region_growing_variants_equal_oracle(lsdgrow_emu, variant, warps):
 # ---------------------------------------------------------------------------------------------------------------------
 @pytest.fixture(scope="module")
 def ba_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libba_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "ba_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("ba_emu", tmp_path_factory, opt="-O1")
 
 
 def _emu_ba_solve(emu, prob, first=5, second=10, mode=0, ctas=3):

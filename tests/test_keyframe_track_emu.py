@@ -5,15 +5,13 @@ then the gather and discard_outliers.  The feature vectors are chosen by the tes
 that every case occurs: empty keyframe nodes, weight-0 words, a node shared by many rows, no shared node, frames that
 do not run the stage, and both status cases.  A second test runs the transform of the active frames only."""
 import ctypes as C
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import emu_build
 import oracle_api
 import synth
-from local_map_data import ROOT
 
 _P = C.c_void_p
 ISIG = synth.inv_level_sigma_sq()
@@ -21,15 +19,7 @@ ISIG = synth.inv_level_sigma_sq()
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libkftrack_emu.so"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-fno-fast-math",
-           "-Wno-subobject-linkage", f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "kftrack_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("kftrack_emu", tmp_path_factory, extra=("-Wno-subobject-linkage",))
 
 
 def _a(x, dt):

@@ -5,7 +5,7 @@
   "det" mode the CUDA path implements and in the "cv" mode (libm, sequential sums).
 * the OpenCV primitives LBD uses (GaussianBlur 5x5 sigma 1, Sobel 3x3 -> CV_16S, LineIterator count) against cv2;
 * LBD itself is vendored reference source (binary_descriptor_custom.cpp) restated line by line: structural checks.
-* detmath (deterministic sin/cos/atan2) against libm, and the two textual copies are identical.
+* detmath (deterministic sin/cos/atan2) against libm.
 """
 import functools
 import math
@@ -210,15 +210,13 @@ def test_line_extract_structure(orc):
     assert len(kl0) == 0
 
 
-def test_detmath_copies_identical_and_accurate(orc):
-    a = (ROOT / "oracle" / "detmath.h").read_text()
-    b = (ROOT / "structure-plp-slam_b200" / "csrc" / "detmath.h").read_text()
-    assert a == b
+def test_detmath_accurate(orc):
     import ctypes as C
     import subprocess
     import tempfile
+    hdr = ROOT / "structure-plp-slam_b200" / "csrc" / "detmath.h"
     src = '#include "%s"\nextern "C" { double t_sin(double x){return det_sin(x);} double t_cos(double x){return det_cos(x);}' \
-          ' double t_atan2(double y,double x){return det_atan2(y,x);} }\n' % (ROOT / "oracle" / "detmath.h")
+          ' double t_atan2(double y,double x){return det_atan2(y,x);} }\n' % hdr
     with tempfile.TemporaryDirectory() as d:
         (Path(d) / "t.cc").write_text(src)
         subprocess.run(["g++", "-O2", "-ffp-contract=off", "-shared", "-fPIC", str(Path(d) / "t.cc"), "-o",

@@ -3,12 +3,11 @@ and gather) executed on the CPU through tests/cta_emu, equal to the oracle chain
 whose local map spans many observe CTAs, a frame whose motion track failed, an empty local map, and both status cases.
 The pose optimiser between gather and finish is the oracle's, run on the observations the emulated gather produced."""
 import ctypes as C
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import emu_build
 import local_map_data as lmd
 import oracle_api
 import scene
@@ -19,16 +18,7 @@ MAX_LOCAL = 2500
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "liblocal_map_emu.so"
-    csrc = lmd.ROOT / "structure-plp-slam_b200" / "csrc"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-fno-fast-math",
-           f"-I{csrc}", f"-I{lmd.ROOT / 'tests' / 'cta_emu'}", str(lmd.ROOT / "tests" / "cta_emu" / "local_map_emu.cc"),
-           "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("local_map_emu", tmp_path_factory)
 
 
 def _a(x, dt):

@@ -1,4 +1,4 @@
-"""CPU tests of the local-map oracle (tests/local_map_oracle.cc + local_map_data's chain): known answers for each
+"""CPU tests of the local-map oracle (oracle/local_map_oracle.cc + local_map_data's chain): known answers for each
 frame::can_observe gate and its boundary values, the exclusion of every landmark the motion track matched (the outliers
 of its pose optimisation included), and the pass-through of frames whose motion track failed."""
 import numpy as np

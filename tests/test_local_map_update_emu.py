@@ -1,15 +1,14 @@
 """The local-map update's DEVICE code (structure-plp-slam_b200/csrc/local_map_update_kernels.cuh) executed on the CPU
 through tests/cta_emu, equal to the Python restatement of update_local_map (tests/local_map_update_data.py), which in
-turn equals the C++ restatement (tests/local_map_update_oracle.cc) list for list.  Batches mix motion-, keyframe- and
+turn equals the C++ restatement (oracle/local_map_update_oracle.cc) list for list.  Batches mix motion-, keyframe- and
 robust-started frames, inactive frames and frames with every status, over band-shaped maps with erased landmarks and
 keyframes, shared landmarks, weight ties, first levels above 60 and lists ending at 61-63."""
 import ctypes as C
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import emu_build
 import local_map_update_data as lmu
 
 _P = C.c_void_p
@@ -33,15 +32,7 @@ class _Map(C.Structure):  # plp_track_map
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "liblmupdate_emu.so"
-    csrc = lmu.ROOT / "structure-plp-slam_b200" / "csrc"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", f"-I{csrc}", f"-I{lmu.ROOT / 'tests' / 'cta_emu'}",
-           str(lmu.ROOT / "tests" / "cta_emu" / "lmupdate_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("lmupdate_emu", tmp_path_factory)
 
 
 def _a(x, dt):

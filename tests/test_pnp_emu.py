@@ -3,28 +3,17 @@ bit-equal to the oracle (oracle/pnp.cc), which compiles the same pnpmath.h text.
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+import emu_build
 import pnp_data as pd
-
-ROOT = Path(__file__).resolve().parents[1]
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libpnp_emu.so"
-    csrc = ROOT / "structure-plp-slam_b200" / "csrc"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-fno-fast-math",
-           f"-I{csrc}", f"-I{ROOT / 'tests' / 'cta_emu'}", str(ROOT / "tests" / "cta_emu" / "pnp_emu.cc"), "-o", str(so)]
-    subprocess.run(cmd, check=True)
-    return C.CDLL(str(so))
+    return emu_build.emu("pnp_emu", tmp_path_factory)
 
 
 def emu_ransac(emu, off, b, x, mc, sm, min_num_inliers=10, recompute=True):

@@ -1,6 +1,6 @@
-"""CPU tests of the solve::pnp_solver restatement (oracle/pnp.cc on pnpmath.h): the textual identity of the two
-pnpmath.h copies, ground-truth recovery on noise-free data, the numpy restatement (numpy's svd / lstsq / inv), OpenCV's
-EPnP frozen in tests/golden/cv2_epnp.npz, the Eigen-replacing helpers, and find_via_ransac's wrapper rules."""
+"""CPU tests of the solve::pnp_solver restatement (oracle/pnp.cc on pnpmath.h): ground-truth recovery on noise-free
+data, the numpy restatement (numpy's svd / lstsq / inv), OpenCV's EPnP frozen in tests/golden/cv2_epnp.npz, the
+Eigen-replacing helpers, and find_via_ransac's wrapper rules."""
 from pathlib import Path
 
 import numpy as np
@@ -10,12 +10,6 @@ import pnp_data as pd
 
 ROOT = Path(__file__).resolve().parent.parent
 GOLDEN = ROOT / "tests" / "golden" / "cv2_epnp.npz"
-
-
-def test_pnpmath_copies_identical():
-    a = (ROOT / "oracle" / "pnpmath.h").read_text()
-    b = (ROOT / "structure-plp-slam_b200" / "csrc" / "pnpmath.h").read_text()
-    assert a == b
 
 
 @pytest.mark.parametrize("seed", range(4))

@@ -3,17 +3,14 @@
 distribute_keypoints_via_tree -- on random candidates (duplicated coordinates, budgets 5 to 1000), on the real FAST
 candidates of every pyramid level, and on a level larger than the shared-memory window (the global-scratch path)."""
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+import emu_build
 import oracle_api
 import synth
 
-ROOT = Path(__file__).resolve().parent.parent
 _P = C.c_void_p
 LEVEL_KP = np.dtype([("x", "<i2"), ("y", "<i2"), ("response", "<i4")])
 PATCH = 19
@@ -21,15 +18,7 @@ PATCH = 19
 
 @pytest.fixture(scope="module")
 def qt_emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libquadtree_emu.so"
-    cmd = ["g++", "-O1", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off",
-           f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / "quadtree_emu.cc"), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("quadtree_emu", tmp_path_factory, opt="-O1")
 
 
 def _slot_cap(w, h, budget):  # orb.cu: initial nodes of the level, one sweep can quadruple them

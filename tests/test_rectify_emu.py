@@ -2,11 +2,11 @@
 tests/cta_emu: the fixed-point map conversion, the tiles, the batch loop and the pitches, equal to the oracle byte for
 byte, with the bytes past `cols` of every output row left as they were."""
 import ctypes as C
-import shutil
 
 import numpy as np
 import pytest
 
+import emu_build
 import rectify_data as rd
 
 _P = C.c_void_p
@@ -14,9 +14,7 @@ _P = C.c_void_p
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    return rd.build_emu(tmp_path_factory.mktemp("emu"))
+    return emu_build.emu("rectify_emu", tmp_path_factory)
 
 
 def _run(emu, mx, my, frames, in_step, out_step):

@@ -1,5 +1,5 @@
 """GPU stereo rectification (plp_stereo_rectifier_*, plp_stereo_rectify, plp_stereo_rectify_batch_dev) against the oracle
-(tests/rectify_oracle.cc, pinned to cv2 by test_rectify_oracle.py), and the device-resident chain raw pair -> rectify ->
+(oracle/rectify_oracle.cc, pinned to cv2 by test_rectify_oracle.py), and the device-resident chain raw pair -> rectify ->
 ORB -> stereo against the oracle chain."""
 import ctypes as C
 import hashlib

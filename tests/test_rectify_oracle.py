@@ -1,4 +1,4 @@
-"""The rectification oracle (tests/rectify_oracle.cc: the maps from structure-plp-slam_b200/csrc/rectmath.h and an
+"""The rectification oracle (oracle/rectify_oracle.cc: the maps from structure-plp-slam_b200/csrc/rectmath.h and an
 independent fixed-point remap) pinned to cv2 bit for bit, and to tests/golden/cv2_rectify.npz without cv2."""
 import hashlib
 from pathlib import Path

@@ -4,44 +4,30 @@ flags, the sample draw of csrc/ransac_sample.h, the match list, the batched hypo
 oracle's essential RANSAC and plp_essential_ransac's device code on the same samples, then the gather and
 discard_outliers.  The brute-force matches are given (the matcher is the existing brute_match_kernel)."""
 import ctypes as C
-import shutil
-import subprocess
 from types import SimpleNamespace
 
 import numpy as np
 import pytest
 
+import emu_build
 import ess_data
 import oracle_api
 import robust_track_data as rtd
 import synth
-from local_map_data import ROOT
 
 _P = C.c_void_p
 ISIG = synth.inv_level_sigma_sq()
 CAM = SimpleNamespace(fx=500.0, fy=505.0, cx=320.5, cy=240.25)
 
 
-def _compile(tmp_path_factory, src, name):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / name
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-fno-fast-math",
-           "-Wno-subobject-linkage", f"-I{ROOT / 'structure-plp-slam_b200' / 'csrc'}", f"-I{ROOT / 'tests' / 'cta_emu'}",
-           str(ROOT / "tests" / "cta_emu" / src), "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
-
-
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    return _compile(tmp_path_factory, "robust_emu.cc", "librobust_emu.so")
+    return emu_build.emu("robust_emu", tmp_path_factory, extra=("-Wno-subobject-linkage",))
 
 
 @pytest.fixture(scope="module")
 def ess_emu(tmp_path_factory):
-    return _compile(tmp_path_factory, "essential_emu.cc", "libessential_emu.so")
+    return emu_build.emu("essential_emu", tmp_path_factory, extra=("-Wno-subobject-linkage",))
 
 
 def _a(x, dt):
@@ -242,7 +228,6 @@ def test_robust_track_kernels_on_cpu_equal_restatement(emu, ess_emu, orc):
     assert num_bf[1] < 8 and valid[1] == 0
     assert valid[2] == 1 and 8 <= num_robust[2] < 20
     assert valid[6] == 1 and num_robust[6] >= 20
-
 
 
 def _run_chain(emu, frames, kfs, kf_of_frame, kf_stage, kf_nv, kf_status, cap, seed):

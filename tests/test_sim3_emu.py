@@ -3,28 +3,17 @@ winning Sim3 bit-equal to the oracle (oracle/sim3.cc), which compiles the same s
 from __future__ import annotations
 
 import ctypes as C
-import shutil
-import subprocess
-from pathlib import Path
 
 import numpy as np
 import pytest
 
+import emu_build
 import sim3_data as sd
-
-ROOT = Path(__file__).resolve().parents[1]
 
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libsim3_emu.so"
-    csrc = ROOT / "structure-plp-slam_b200" / "csrc"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-fno-fast-math",
-           f"-I{csrc}", f"-I{ROOT / 'tests' / 'cta_emu'}", str(ROOT / "tests" / "cta_emu" / "sim3_emu.cc"), "-o", str(so)]
-    subprocess.run(cmd, check=True)
-    return C.CDLL(str(so))
+    return emu_build.emu("sim3_emu", tmp_path_factory)
 
 
 def emu_ransac(emu, off, x1, x2, c1, c2, sm, fix_scale=False, min_num_inliers=20):

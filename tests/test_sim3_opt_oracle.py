@@ -4,8 +4,6 @@ the group operations against 4 x 4 similarity matrices, the numeric Jacobian aga
 optimum against scipy.optimize.least_squares on the same robust cost, and the reference's control flow."""
 from __future__ import annotations
 
-from pathlib import Path
-
 import numpy as np
 import pytest
 from scipy.linalg import expm
@@ -13,8 +11,6 @@ from scipy.optimize import least_squares
 from scipy.spatial.transform import Rotation
 
 import sim3_opt_data as sd
-
-ROOT = Path(__file__).resolve().parents[1]
 
 
 def generator(u):
@@ -24,12 +20,6 @@ def generator(u):
     G[:3, :3] = np.array([[0, -w[2], w[1]], [w[2], 0, -w[0]], [-w[1], w[0], 0]]) + sg * np.eye(3)
     G[:3, 3] = v
     return G
-
-
-def test_math_header_copies_identical():
-    a = (ROOT / "oracle" / "sim3optmath.h").read_bytes()
-    b = (ROOT / "structure-plp-slam_b200" / "csrc" / "sim3optmath.h").read_bytes()
-    assert a == b
 
 
 # theta and sigma on both sides of g2o's eps = 1e-5 (and exactly zero)

@@ -2,21 +2,11 @@
 the numpy restatement in tests/sim3_data.py, plus the reference's boundaries and sim3math.h's two deviations."""
 from __future__ import annotations
 
-from pathlib import Path
-
 import numpy as np
 import pytest
 from scipy.spatial.transform import Rotation
 
 import sim3_data as sd
-
-ROOT = Path(__file__).resolve().parents[1]
-
-
-def test_math_header_copies_are_identical():
-    a = (ROOT / "oracle" / "sim3math.h").read_bytes()
-    b = (ROOT / "structure-plp-slam_b200" / "csrc" / "sim3math.h").read_bytes()
-    assert a == b
 
 
 @pytest.mark.parametrize("fix_scale,scale", [(False, 2.0), (False, 0.5), (True, None)])

@@ -4,12 +4,11 @@ gather (track_common.cuh) with the current frames' x_right, and the local-map st
 x_right_in_tracking_ and the matcher's x_right gate.  Observations are compared with the arrays pose_optimizer.cc:126-151
 builds: x_right >= 0 is a stereo edge (0 included), < 0 a 2-D edge."""
 import ctypes as C
-import shutil
-import subprocess
 
 import numpy as np
 import pytest
 
+import emu_build
 import local_map_data as lmd
 import oracle_api
 import scene
@@ -23,16 +22,7 @@ BF = 40.0
 
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
-    if shutil.which("g++") is None:
-        pytest.skip("g++ not available")
-    so = tmp_path_factory.mktemp("emu") / "libstereo_track_emu.so"
-    csrc = lmd.ROOT / "structure-plp-slam_b200" / "csrc"
-    cmd = ["g++", "-O2", "-std=c++17", "-pthread", "-shared", "-fPIC", "-ffp-contract=off", "-fno-fast-math",
-           f"-I{csrc}", f"-I{lmd.ROOT / 'tests' / 'cta_emu'}", str(lmd.ROOT / "tests" / "cta_emu" / "stereo_track_emu.cc"),
-           "-o", str(so)]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    assert res.returncode == 0, res.stderr[:3000]
-    return C.CDLL(str(so))
+    return emu_build.emu("stereo_track_emu", tmp_path_factory)
 
 
 def _a(x, dt):

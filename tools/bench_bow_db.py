@@ -1,6 +1,6 @@
 """Times plp_bow_db relocalisation queries: 512 queries per batch against K keyframes whose bow_vec_ hold ~1000 words
 drawn from a scene vocabulary, for K in {128, 1000, 10000}.  The device time is the host entry's wall time (upload of
-the queries and graph, the query kernel, download).  The host column is the C++ restatement (tests/bow_db_oracle.cc,
+the queries and graph, the query kernel, download).  The host column is the C++ restatement (oracle/bow_db_oracle.cc,
 -O3, the reference's containers) on one thread over the same 512 queries.  Also timed: adding all K keyframes in one
 call, and, on the full database, erasing one keyframe and adding it back (the mapping thread's per-keyframe cost).
 Prints the card's name and power limit from the same run.
@@ -13,7 +13,6 @@ import argparse
 import json
 import subprocess
 import sys
-import tempfile
 import time
 from pathlib import Path
 
@@ -46,7 +45,7 @@ def main():
     voc = plp.capi.BowVocabulary(ctx, k=v["k"], L=v["L"], parent=v["parent"], desc=v["desc"], weight=v["weight"],
                                  is_leaf=v["is_leaf"])
     nw = voc.info()["num_words"]
-    orc = bdd.build_oracle(tempfile.mkdtemp(prefix="bow_db_oracle_"))
+    orc = bdd.oracle()
     rng = np.random.default_rng(0)
     scene_words = np.sort(rng.choice(nw, size=min(nw, 8000), replace=False))  # the words one scene uses
     print(f"card: {card()}; vocabulary words: {nw}; scene words: {len(scene_words)}")

@@ -7,7 +7,7 @@ tracking on a high-priority tracking context) over a 128-keyframe map snapshot
 (tests/local_map_update_data.bench_snapshot).  The script
   1. checks the device update of every frame against the restatement of update_local_map;
   2. times, alternately, step + update_local_map + track_local_map on the device list, and step + the host path
-     (synchronise, download the matches, the native graph walk of tests/local_map_update_oracle.cc over the batch,
+     (synchronise, download the matches, the native graph walk of oracle/local_map_update_oracle.cc over the batch,
      gather and upload the lists and the row mappings) + track_local_map on the uploaded list, each part timed, with a
      device synchronise around each timed step;
   3. times the update's kernels (plp_ctx_kernel_timing) over further update_local_map() calls.
