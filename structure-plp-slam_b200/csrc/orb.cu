@@ -140,47 +140,108 @@ __device__ __forceinline__ void tma_box_load(uint32_t dst, const CUtensorMap *tm
 // =====================================================================================================
 // 1. pyramid: cv::resize(INTER_LINEAR) fixed-point model (SURVEY.md Appendix A.1)
 // =====================================================================================================
-// tables: per destination column {sx0, sx1, a0, a1}, per destination row {sy0, sy1, b0, b1}
-// A thread owns four destination columns of kResizeRows consecutive rows: the column taps and weights are row-independent,
-// so they are unpacked once per strip (round 1 redid the table loads, the unpacking and the 64-bit address arithmetic for
-// every row: 58 instructions per pixel).
-constexpr int kResizeRows = 8;
-__global__ void __launch_bounds__(256) pyr_resize_kernel(OrbDev P, int l, const short4 *__restrict__ xtab,
-                                                         const short4 *__restrict__ ytab) {
-    const int b = blockIdx.y;
-    const int dw = P.lv[l].w, dh = P.lv[l].h, dpitch = P.lv[l].pitch;
-    const int quads = (dw + 3) >> 2, strips = (dh + kResizeRows - 1) / kResizeRows;
-    const int q = blockIdx.x * blockDim.x + threadIdx.x;
-    if (q >= quads * strips) return;
-    const int strip = q / quads, x0 = (q - strip * quads) * 4;
-    const uint8_t *src = level_ptr(P, b, l - 1);
-    const int spitch = level_pitch(P, l - 1);
-    uint8_t *dst = const_cast<uint8_t *>(level_ptr(P, b, l));
-    int sx0[4], sx1[4], a0[4], a1[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-        const short4 xt = xtab[min(x0 + k, dw - 1)];  // columns past dw are row padding: any value may be stored there
-        sx0[k] = xt.x;
-        sx1[k] = xt.y;
-        a0[k] = xt.z;
-        a1[k] = xt.w;
-    }
-    const int y_end = min(dh, (strip + 1) * kResizeRows);
-    for (int y = strip * kResizeRows; y < y_end; ++y) {
-        const short4 yt = ytab[y];
-        const uint8_t *S0 = src + (size_t)yt.x * spitch, *S1 = src + (size_t)yt.y * spitch;
-        const int b0 = yt.z, b1 = yt.w;
-        uint32_t packed = 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const int r0 = S0[sx0[k]] * a0[k] + S0[sx1[k]] * a1[k];
-            const int r1 = S1[sx0[k]] * a0[k] + S1[sx1[k]] * a1[k];
-            const int v = (((b0 * (r0 >> 4)) >> 16) + ((b1 * (r1 >> 4)) >> 16) + 2) >> 2;
-            packed |= (uint32_t)(v & 0xff) << (8 * k);
+// tables: per destination column {sx0, sx1, a0, a1} (padded to a multiple of 16 columns with copies of the last one),
+// per destination row {sy0, sy1, b0, b1}.  The resize is separable: h[x] = (S[sx0]·a0 + S[sx1]·a1) >> 4 (at most
+// 32 640, a uint16) is computed once per source row, and v = (((b0·h0) >> 16) + ((b1·h1) >> 16) + 2) >> 2 once per
+// destination pixel from the two rows' h.  A destination row band stages its source rows [sy0(first), sy1(last)] in
+// shared memory with 16-byte copies, builds their h rows there and writes 8 destination bytes per store; bytes past
+// the level width are row padding (the pitch is a multiple of 64, the h rows a multiple of 16 columns).
+// Shared-memory rows: a staged source row of width w takes pad16(w) bytes, an h row of width w pad16(w) uint16.
+__host__ __device__ __forceinline__ int pad16(int w) { return (w + 15) & ~15; }
+
+// f(r, g) for every r < rows, g < cols, spread over the CTA's threads (row-major; one division per thread)
+template <class F>
+__device__ __forceinline__ void cta_for_2d(int rows, int cols, F f) {
+    const int nth = blockDim.x, dr = nth / cols, dg = nth - dr * cols;
+    for (int r = threadIdx.x / cols, g = threadIdx.x - (threadIdx.x / cols) * cols; r < rows;) {
+        f(r, g);
+        g += dg;
+        r += dr;
+        if (g >= cols) {
+            g -= cols;
+            ++r;
         }
-        // pitch is a multiple of 64 so the 4-byte store is aligned; pad bytes past dw are never read
-        *reinterpret_cast<uint32_t *>(dst + (size_t)y * dpitch + x0) = packed;
     }
+}
+
+// rows [s0, s0 + ns) of a w-wide level (global, `pitch`) -> shared memory at pitch pad16(w).  16-byte cp.async copies,
+// all of a thread's in flight at once, when the level's base and pitch allow them (always for the levels in d_pyr; the
+// caller's level 0 may be pitched oddly), byte loads otherwise.
+__device__ __forceinline__ void stage_rows(uint8_t *S, const uint8_t *src, size_t pitch, int w, int s0, int ns) {
+    const int sp = pad16(w);
+    src += (size_t)s0 * pitch;
+    if ((((uintptr_t)src | pitch) & 15) == 0) {  // then pitch >= pad16(w): no copy leaves the row
+        cta_for_2d(ns, sp >> 4, [&](int r, int c) {
+            asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(S + r * sp + 16 * c)),
+                         "l"(src + r * pitch + 16 * c)
+                         : "memory");
+        });
+        asm volatile("cp.async.wait_all;" ::: "memory");
+    } else {
+        cta_for_2d(ns, w, [&](int r, int x) { S[r * sp + x] = src[r * pitch + x]; });
+    }
+}
+
+// horizontal pass: h rows [0, ns) from staged source rows [0, ns).  A thread owns a pair of columns (the CTA is sized
+// to the level's width, pyr_threads) and walks down the rows with its taps in registers; a warp's byte gathers fall
+// within ~80 consecutive bytes of a row (no bank conflicts)
+__device__ __forceinline__ void resize_rows_h(uint16_t *H, const uint8_t *S, int sw, int ns, int dw,
+                                              const short4 *__restrict__ xtab) {
+    const int sp = pad16(sw), hw = pad16(dw) >> 1;  // h rows in 32-bit words (2 columns each)
+    for (int g = threadIdx.x; g < hw; g += blockDim.x) {
+        const uint4 t = __ldg(reinterpret_cast<const uint4 *>(xtab + 2 * g));  // {sx0 | sx1 << 16, a0 | a1 << 16} x 2
+        const int x00 = t.x & 0xffff, x01 = t.x >> 16, x10 = t.z & 0xffff, x11 = t.z >> 16;
+        const int a00 = t.y & 0xffff, a01 = t.y >> 16, a10 = t.w & 0xffff, a11 = t.w >> 16;
+        const uint8_t *s = S;
+        uint32_t *h = reinterpret_cast<uint32_t *>(H) + g;
+#pragma unroll 4
+        for (int r = 0; r < ns; ++r, s += sp, h += hw) {
+            const uint32_t h0 = (s[x00] * a00 + s[x01] * a01) >> 4;
+            const uint32_t h1 = (s[x10] * a10 + s[x11] * a11) >> 4;
+            *h = h0 | h1 << 16;
+        }
+    }
+}
+
+// vertical pass: destination rows [y0, y1) from the h rows of source rows [s0, ...), 8 columns per item (conflict-free
+// 16-byte shared loads, coalesced 8-byte stores) to `dst` (global, `dpitch`)
+__device__ __forceinline__ uint32_t resize_v4(int b0, int b1, uint32_t p0, uint32_t q0, uint32_t p1, uint32_t q1) {
+    const int v0 = (((b0 * (int)(p0 & 0xffff)) >> 16) + ((b1 * (int)(p1 & 0xffff)) >> 16) + 2) >> 2;
+    const int v1 = (((b0 * (int)(p0 >> 16)) >> 16) + ((b1 * (int)(p1 >> 16)) >> 16) + 2) >> 2;
+    const int v2 = (((b0 * (int)(q0 & 0xffff)) >> 16) + ((b1 * (int)(q1 & 0xffff)) >> 16) + 2) >> 2;
+    const int v3 = (((b0 * (int)(q0 >> 16)) >> 16) + ((b1 * (int)(q1 >> 16)) >> 16) + 2) >> 2;
+    return (uint32_t)(v0 & 0xff) | (uint32_t)(v1 & 0xff) << 8 | (uint32_t)(v2 & 0xff) << 16 | (uint32_t)(v3 & 0xff) << 24;
+}
+__device__ __forceinline__ void resize_rows_v(uint8_t *dst, int dpitch, const uint16_t *H, int s0, int y0, int y1, int dw,
+                                              const short4 *__restrict__ ytab) {
+    const int hp = pad16(dw);
+    cta_for_2d(y1 - y0, hp >> 3, [&](int r, int g) {
+        const int y = y0 + r;
+        const short4 yt = __ldg(ytab + y);
+        const uint4 a = *reinterpret_cast<const uint4 *>(H + (yt.x - s0) * hp + 8 * g);
+        const uint4 e = *reinterpret_cast<const uint4 *>(H + (yt.y - s0) * hp + 8 * g);
+        *reinterpret_cast<uint2 *>(dst + (size_t)y * dpitch + 8 * g) =
+            make_uint2(resize_v4(yt.z, yt.w, a.x, a.y, e.x, e.y), resize_v4(yt.z, yt.w, a.z, a.w, e.z, e.w));
+    });
+}
+
+// level l from level l-1, one band of `band` destination rows per CTA (blockIdx.x), frame blockIdx.y
+constexpr int kPyrMaxThreads = 1024;
+__global__ void __launch_bounds__(kPyrMaxThreads) pyr_resize_kernel(OrbDev P, int l, int band,
+                                                                    const short4 *__restrict__ xtab,
+                                                                    const short4 *__restrict__ ytab) {
+    extern __shared__ __align__(16) uint8_t smem[];
+    const int b = blockIdx.y;
+    const int sw = P.lv[l - 1].w, dw = P.lv[l].w, dh = P.lv[l].h;
+    const int y0 = blockIdx.x * band, y1 = min(dh, y0 + band);
+    const int s0 = __ldg(&ytab[y0].x), ns = __ldg(&ytab[y1 - 1].y) - s0 + 1;
+    uint8_t *S = smem;
+    uint16_t *H = reinterpret_cast<uint16_t *>(smem + ns * pad16(sw));
+    stage_rows(S, level_ptr(P, b, l - 1), level_pitch(P, l - 1), sw, s0, ns);
+    __syncthreads();
+    resize_rows_h(H, S, sw, ns, dw, xtab);
+    __syncthreads();
+    resize_rows_v(const_cast<uint8_t *>(level_ptr(P, b, l)), P.lv[l].pitch, H, s0, y0, y1, dw, ytab);
 }
 
 // =====================================================================================================
@@ -1047,6 +1108,9 @@ struct plp_orb {
     std::vector<CellDesc> cells;
     short4 *d_xtab[kMaxLevels] = {nullptr};
     short4 *d_ytab[kMaxLevels] = {nullptr};
+    // pyr_resize_kernel builds level l in bands of pyr_band[l] rows (0: an empty level, not built), pyr_threads[l] per CTA
+    int pyr_band[kMaxLevels] = {0}, pyr_threads[kMaxLevels] = {0};
+    size_t pyr_band_smem[kMaxLevels] = {0};
     CellDesc *d_cells = nullptr;
     uint8_t *d_pyr = nullptr;
     uint8_t *d_blur = nullptr;
@@ -1104,6 +1168,21 @@ static bool encode_level_map(CUtensorMap *m, const uint8_t *base, int w, int h, 
                CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
+
+// pyr_resize_kernel: rows per band, halved until a band's staged source rows and h rows fit kPyrBandSmem (several
+// CTAs per SM)
+constexpr int kPyrBandRows = 16;
+constexpr size_t kPyrBandSmem = 48 * 1024;
+
+// the most source rows a band of `band` destination rows reads
+static int band_src_rows(const std::vector<short4> &yt, int band) {
+    int m = 0;
+    for (int y0 = 0; y0 < (int)yt.size(); y0 += band) {
+        const int y1 = std::min((int)yt.size(), y0 + band);
+        m = std::max(m, yt[y1 - 1].y - yt[y0].x + 1);
+    }
+    return m;
+}
 
 static void build_resize_tables(int sw, int sh, int dw, int dh, std::vector<short4> &xt, std::vector<short4> &yt) {
     // cv::resize INTER_LINEAR 8U: 11-bit coefficients, rounded half-to-even (SURVEY.md Appendix A.1)
@@ -1332,13 +1411,26 @@ plp_status plp_orb_create(plp_ctx *ctx, const plp_orb_params *params, int rows, 
             return PLP_ERR_CUDA;                                           \
         }                                                                  \
     } while (0)
+    // pyramid tables and work split; a level of zero width or height (and every level after it) is not built
+    size_t pyr_band_smem_max = 0;
     for (unsigned l = 1; l < L; ++l) {
+        const LevelInfo &S = D.lv[l - 1], &V = D.lv[l];
+        if (V.w < 1 || V.h < 1) break;
         std::vector<short4> xt, yt;
-        build_resize_tables(D.lv[l - 1].w, D.lv[l - 1].h, D.lv[l].w, D.lv[l].h, xt, yt);
+        build_resize_tables(S.w, S.h, V.w, V.h, xt, yt);
+        const short4 last = xt.back();
+        xt.resize(pad16(V.w), last);  // the kernel builds h rows of pad16(w) columns
         ORB_ALLOC(o->d_xtab[l], xt.size() * sizeof(short4));
         ORB_ALLOC(o->d_ytab[l], yt.size() * sizeof(short4));
         cudaMemcpy(o->d_xtab[l], xt.data(), xt.size() * sizeof(short4), cudaMemcpyHostToDevice);
         cudaMemcpy(o->d_ytab[l], yt.data(), yt.size() * sizeof(short4), cudaMemcpyHostToDevice);
+        const size_t row_bytes = pad16(S.w) + 2 * pad16(V.w);
+        int band = kPyrBandRows;
+        while (band > 1 && band_src_rows(yt, band) * row_bytes > kPyrBandSmem) band >>= 1;
+        o->pyr_band[l] = band;
+        o->pyr_threads[l] = std::min(kPyrMaxThreads, (pad16(V.w) / 2 + 31) & ~31);  // one thread per h column pair
+        o->pyr_band_smem[l] = band_src_rows(yt, band) * row_bytes;
+        pyr_band_smem_max = std::max(pyr_band_smem_max, o->pyr_band_smem[l]);
     }
     ORB_ALLOC(o->d_cells, o->cells.size() * sizeof(CellDesc));
     if (!o->cells.empty())
@@ -1378,7 +1470,11 @@ plp_status plp_orb_create(plp_ctx *ctx, const plp_orb_params *params, int rows, 
         o->maps_ok = encode_level_map(&o->maps.m[l], o->d_pyr + D.lv[l].offset, D.lv[l].w, D.lv[l].h, max_batch, D.lv[l].pitch,
                                       D.pyr_frame_bytes);
     o->qt_small = qt_max_slots <= kNodeCapSmall;
-    plp_status so;
+    plp_status so = ensure_smem_optin((const void *)pyr_resize_kernel, pyr_band_smem_max, "pyr_resize_kernel");
+    if (so != PLP_OK) {
+        plp_orb_destroy(o);
+        return so;
+    }
     if (o->qt_small) {
         o->qt_smem = qt_smem_bytes<kNodeCapSmall, kCandCapSmall, kQtThreadsSmall>();
         so = ensure_smem_optin((const void *)kQtSmall, o->qt_smem, "quadtree_kernel<small>");
@@ -1422,11 +1518,10 @@ static plp_status orb_run(plp_orb *o, const uint8_t *d_imgs, int batch, size_t s
     o->last_img0 = d_imgs;
     o->last_step = step;
     PLP_CUDA_TRY(cudaMemsetAsync(D.status, 0, (size_t)batch * sizeof(int), ctx->stream));
-    for (int l = 1; l < D.num_levels; ++l) {
-        const int quads = ((D.lv[l].w + 3) >> 2) * ((D.lv[l].h + kResizeRows - 1) / kResizeRows);  // threads: 4 columns x 8 rows each
-        if (quads <= 0) continue;
-        dim3 grid(div_up(quads, 256), batch);
-        PLP_LAUNCH(ctx, pyr_resize_kernel, grid, 256, 0, D, l, o->d_xtab[l], o->d_ytab[l]);
+    for (int l = 1; l < D.num_levels && o->pyr_band[l] > 0; ++l) {
+        dim3 grid(div_up(D.lv[l].h, o->pyr_band[l]), batch);
+        PLP_LAUNCH(ctx, pyr_resize_kernel, grid, o->pyr_threads[l], o->pyr_band_smem[l], D, l, o->pyr_band[l], o->d_xtab[l],
+                   o->d_ytab[l]);
     }
     // TMA descriptors for the FAST tiles and the blur boxes: level 0 is the caller's buffer
     bool tma = o->maps_ok;
